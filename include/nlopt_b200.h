@@ -268,6 +268,10 @@ typedef struct {
     double seconds_dual_wall;    /* wall: inside dual solves (launch to result, incl. exchange)    */
     double seconds_eval_wall;    /* wall: objective + constraint evaluations (callbacks + copies)  */
     double seconds_glue_wall;    /* wall: sigma init, end-of-outer pass, final copy of x           */
+    long long dual_operand_bytes; /* HBM bytes the dual kernels were asked to read on this rank, summed over evaluations,
+                                     plus their stores of x*(y): 8 ld (3 + m) per evaluation when both bounds are
+                                     uniform (nlopt_set_*_bounds1) and the default kernels run, 8 ld (5 + m) otherwise;
+                                     ld = this rank's padded shard length */
 } nlopt_b200_stats;
 nlopt_result nlopt_b200_get_stats(const nlopt_opt opt, nlopt_b200_stats *out);
 

@@ -276,6 +276,7 @@ struct DualArgs {
     double rho, half_rho, u_ccsaq;    // u_ccsaq = rho + sum_i rhoc_i y_i (ccsa_quadratic.c:116-120)
     double y[kMaxParamM], rhoc[kMaxParamM], half_rhoc[kMaxParamM];       // (m <= 16)
     const double *wide;           // m > 16: device block  y[m] | rhoc[m] | half_rhoc[m] | active[m] (1.0 / 0.0)
+    double lb_u, ub_u;            // the value of every lb / ub entry when both are uniform (read by the SB instantiations)
     __device__ __forceinline__ double u() const { return u_ccsaq; }
 };
 
@@ -692,7 +693,10 @@ __device__ __noinline__ void eval_folder(const DualArgs &a, int nv_total)
 // Sweep one group: this warp's lanes of every chunk of group `gl`, m+3 lane accumulators.
 // POL: load through the per-array L2 cache policies (persistent solve kernel with b200_l2_keep_mb), else plain
 // streaming loads.
-template <int VARIANT, int MAXM, bool FULL, int UNROLL, bool POL, class MU>
+// SB ("scalar bounds"): every lb entry equals a.lb_u and every ub entry a.ub_u (box bounds set with
+// nlopt_set_*_bounds1).  The two arrays are not read: 3 + m operand arrays per evaluation instead of 5 + m.  The
+// closed forms receive the same values as from the arrays, so the results are the same bits.
+template <int VARIANT, int MAXM, bool FULL, int UNROLL, bool POL, bool SB, class MU>
 __device__ __forceinline__ void sweep_group(const DualArgs &a, const MU &mu, const L2Policies &pol, bool store, unsigned gl, int sub,
                                             int lane, double (&acc)[3 + (MAXM > 0 ? MAXM : 1)])
 {
@@ -718,11 +722,16 @@ __device__ __forceinline__ void sweep_group(const DualArgs &a, const MU &mu, con
             const bool live = u == 0 || p < p_hi;
             vs[u] = make_double2(0.0, 0.0);      // sigma = 0 lanes are skipped by both formulas
             vx[u] = vlb[u] = vub[u] = vg[u] = make_double2(0.0, 0.0);
+            if (SB) {
+                vlb[u] = make_double2(a.lb_u, a.lb_u);
+                vub[u] = make_double2(a.ub_u, a.ub_u);
+            }
             if (live) {
                 if (POL && pol.l1pf && u == UNROLL - 1) {
                     const unsigned long long pn = p + kChunkPairs;                  // this lane's pair of the next chunk
                     if (pn < p_hi) {
-                        prefetch_l1(x2 + pn); prefetch_l1(lb2 + pn); prefetch_l1(ub2 + pn); prefetch_l1(s2v + pn); prefetch_l1(g2 + pn);
+                        prefetch_l1(x2 + pn); prefetch_l1(s2v + pn); prefetch_l1(g2 + pn);
+                        if (!SB) { prefetch_l1(lb2 + pn); prefetch_l1(ub2 + pn); }
 #pragma unroll
                         for (int i = 0; i < MR; ++i)
                             if (MAXM > 0 && (FULL || i < mu.m))
@@ -730,10 +739,12 @@ __device__ __forceinline__ void sweep_group(const DualArgs &a, const MU &mu, con
                     }
                 }
                 if (POL) {
-                    vx[u] = pol.ld(x2 + p, 0); vlb[u] = pol.ld(lb2 + p, 1); vub[u] = pol.ld(ub2 + p, 2);
+                    vx[u] = pol.ld(x2 + p, 0);
+                    if (!SB) { vlb[u] = pol.ld(lb2 + p, 1); vub[u] = pol.ld(ub2 + p, 2); }
                     vs[u] = pol.ld(s2v + p, 3); vg[u] = pol.ld(g2 + p, 4);
                 } else {
-                    vx[u] = ld_stream(x2 + p); vlb[u] = ld_stream(lb2 + p); vub[u] = ld_stream(ub2 + p);
+                    vx[u] = ld_stream(x2 + p);
+                    if (!SB) { vlb[u] = ld_stream(lb2 + p); vub[u] = ld_stream(ub2 + p); }
                     vs[u] = ld_stream(s2v + p); vg[u] = ld_stream(g2 + p);
                 }
             }
@@ -786,13 +797,17 @@ struct ChunkOperands {
     double Ga[MAXM > 0 ? MAXM : 1], Gb[MAXM > 0 ? MAXM : 1];
 };
 
-template <int MAXM, bool FULL, bool POL>
+template <int MAXM, bool FULL, bool POL, bool SB>
 __device__ __forceinline__ void load_chunk(const DualArgs &a, int m, const L2Policies &pol, unsigned long long p, bool live,
                                            ChunkOperands<MAXM> &r)
 {
     constexpr int MR = MAXM > 0 ? MAXM : 1;
     r.s = make_double2(0.0, 0.0);                 // sigma = 0 lanes are skipped by both formulas
     r.x = r.lb = r.ub = r.g = make_double2(0.0, 0.0);
+    if (SB) {                                     // uniform bounds (see sweep_group): no lb / ub loads
+        r.lb = make_double2(a.lb_u, a.lb_u);
+        r.ub = make_double2(a.ub_u, a.ub_u);
+    }
     if (live) {
         const double2 *x2 = reinterpret_cast<const double2 *>(a.x) + p;
         const double2 *lb2 = reinterpret_cast<const double2 *>(a.lb) + p;
@@ -800,9 +815,13 @@ __device__ __forceinline__ void load_chunk(const DualArgs &a, int m, const L2Pol
         const double2 *s2v = reinterpret_cast<const double2 *>(a.sigma) + p;
         const double2 *g2 = reinterpret_cast<const double2 *>(a.g) + p;
         if (POL) {
-            r.x = pol.ld(x2, 0); r.lb = pol.ld(lb2, 1); r.ub = pol.ld(ub2, 2); r.s = pol.ld(s2v, 3); r.g = pol.ld(g2, 4);
+            r.x = pol.ld(x2, 0);
+            if (!SB) { r.lb = pol.ld(lb2, 1); r.ub = pol.ld(ub2, 2); }
+            r.s = pol.ld(s2v, 3); r.g = pol.ld(g2, 4);
         } else {
-            r.x = ld_stream(x2); r.lb = ld_stream(lb2); r.ub = ld_stream(ub2); r.s = ld_stream(s2v); r.g = ld_stream(g2);
+            r.x = ld_stream(x2);
+            if (!SB) { r.lb = ld_stream(lb2); r.ub = ld_stream(ub2); }
+            r.s = ld_stream(s2v); r.g = ld_stream(g2);
         }
     }
 #pragma unroll
@@ -844,7 +863,7 @@ __device__ __forceinline__ double2 compute_chunk(const MU &mu, const DivBy &U, c
 }
 
 // the rest of a group whose first chunk (pair index p_first of this lane, `first`) is already on its way
-template <int VARIANT, int MAXM, bool FULL, bool POL, bool PAIR_MMA, class MU>
+template <int VARIANT, int MAXM, bool FULL, bool POL, bool PAIR_MMA, bool SB, class MU>
 __device__ __forceinline__ void sweep_group_preloaded(const DualArgs &a, const MU &mu, const L2Policies &pol, bool store,
                                                       unsigned long long p_first, unsigned long long p_hi, ChunkOperands<MAXM> &r,
                                                       double (&acc)[3 + (MAXM > 0 ? MAXM : 1)])
@@ -861,7 +880,7 @@ __device__ __forceinline__ void sweep_group_preloaded(const DualArgs &a, const M
         if (store) st_stream(reinterpret_cast<double2 *>(a.xcur) + p, xc);
         p += kChunkPairs;
         live = p < p_hi;
-        if (live) load_chunk<MAXM, FULL, POL>(a, mu.m, pol, p, true, r);
+        if (live) load_chunk<MAXM, FULL, POL, SB>(a, mu.m, pol, p, true, r);
     }
 }
 
@@ -875,6 +894,7 @@ __device__ __forceinline__ void prefetch_l2_bulk(const void *p, unsigned bytes)
     asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
 }
 // called by ONE thread: the bulk prefetch is a uniform-datapath instruction (UBLKPF), one array per issue
+template <bool SB>
 __device__ __forceinline__ void prefetch_group_head(const DualArgs &a, unsigned gl, unsigned chunks)
 {
     unsigned long long p_lo, p_hi;
@@ -884,8 +904,10 @@ __device__ __forceinline__ void prefetch_group_head(const DualArgs &a, unsigned 
     if (np == 0) return;
     const unsigned bytes = (unsigned) (np * 16);
     prefetch_l2_bulk(a.x + 2 * p_lo, bytes);
-    prefetch_l2_bulk(a.lb + 2 * p_lo, bytes);
-    prefetch_l2_bulk(a.ub + 2 * p_lo, bytes);
+    if (!SB) {
+        prefetch_l2_bulk(a.lb + 2 * p_lo, bytes);
+        prefetch_l2_bulk(a.ub + 2 * p_lo, bytes);
+    }
     prefetch_l2_bulk(a.sigma + 2 * p_lo, bytes);
     prefetch_l2_bulk(a.g + 2 * p_lo, bytes);
     for (int i = 0; i < a.m; ++i) prefetch_l2_bulk(a.G + (unsigned long long) i * a.ld + 2 * p_lo, bytes);
@@ -904,7 +926,7 @@ __device__ __forceinline__ void put_group_record(const double *srec, double *gro
     }
 }
 
-template <int VARIANT, int MAXM, bool FULL, bool STORE, int BLOCK, int UNROLL, int MINB>
+template <int VARIANT, int MAXM, bool FULL, bool STORE, int BLOCK, int UNROLL, int MINB, bool SB>
 __global__ void __launch_bounds__(BLOCK, MINB) dual_eval_kernel(const __grid_constant__ DualArgs a)
 {
     constexpr int MR = MAXM > 0 ? MAXM : 1;
@@ -926,7 +948,7 @@ __global__ void __launch_bounds__(BLOCK, MINB) dual_eval_kernel(const __grid_con
         double acc[NV];
 #pragma unroll
         for (int k = 0; k < NV; ++k) acc[k] = 0.0;
-        sweep_group<VARIANT, MAXM, FULL, UNROLL, false>(a, a, pol, STORE, gl, sub, lane, acc);   // multipliers = the parameter block itself
+        sweep_group<VARIANT, MAXM, FULL, UNROLL, false, SB>(a, a, pol, STORE, gl, sub, lane, acc);   // multipliers = the parameter block itself
 
         // warp record -> shared memory; one CTA barrier per group; the record buffer is double-buffered across
         // iterations so the next group's writers can never overtake this group's reader.
@@ -1645,7 +1667,7 @@ __device__ __noinline__ void solve_folder(const SolveArgs &sa, double *s_vs, dou
     }
 }
 
-template <int VARIANT, int MAXM, bool FULL, bool POL, int BLOCK, int UNROLL, int MINB>
+template <int VARIANT, int MAXM, bool FULL, bool POL, int BLOCK, int UNROLL, int MINB, bool SB>
 __global__ void __launch_bounds__(BLOCK, MINB) dual_solve_kernel(const __grid_constant__ SolveArgs sa)
 {
     constexpr int MR = MAXM > 0 ? MAXM : 1;
@@ -1691,12 +1713,12 @@ __global__ void __launch_bounds__(BLOCK, MINB) dual_solve_kernel(const __grid_co
         group_pairs(a.nchunks, a.nseg_total, a.chunk0, a.seg0 + gl, &p_lo, &p_hi);
         const unsigned long long p_first = p_lo + sub * 32 + lane;
         ChunkOperands<MAXM> first;
-        load_chunk<MAXM, FULL, POL>(a, a.m, pol, p_first, p_first < p_hi, first);
+        load_chunk<MAXM, FULL, POL, SB>(a, a.m, pol, p_first, p_first < p_hi, first);
 #endif
         // wait until generation `want` is published (or the solve has finished); refresh the multipliers
         if (want != my_gen) {
             // ... with the head of the group on its way from HBM to the L2 meanwhile
-            if (threadIdx.x == 32 && a.prefetch_chunks) prefetch_group_head(a, gl, a.prefetch_chunks);
+            if (threadIdx.x == 32 && a.prefetch_chunks) prefetch_group_head<SB>(a, gl, a.prefetch_chunks);
             if (sub == 0) {                   // warp 0 polls, warp-uniformly: lane i < m: y_i, lane m: u, the others: flags
                 const int slot = lane < a.m ? lane : (lane == a.m ? kMaxParamM : kMaxParamM + 1);
                 const unsigned long long tag = sa.tag0 | want;
@@ -1743,9 +1765,9 @@ __global__ void __launch_bounds__(BLOCK, MINB) dual_solve_kernel(const __grid_co
         NB_TR(const unsigned long long tr_s0 = nb_globaltimer();)
 #if NB200_PRELOAD
         // (the 128-register instantiations, MINB <= 2, have room for the MMA pair form with 4 rows)
-        sweep_group_preloaded<VARIANT, MAXM, FULL, POL, kPairMMA<MAXM> || (MINB <= 2 && MAXM <= 4)>(a, mu, pol, s_store != 0, p_first, p_hi, first, acc);
+        sweep_group_preloaded<VARIANT, MAXM, FULL, POL, kPairMMA<MAXM> || (MINB <= 2 && MAXM <= 4), SB>(a, mu, pol, s_store != 0, p_first, p_hi, first, acc);
 #else
-        sweep_group<VARIANT, MAXM, FULL, UNROLL, POL>(a, mu, pol, s_store != 0, gl, sub, lane, acc);
+        sweep_group<VARIANT, MAXM, FULL, UNROLL, POL, SB>(a, mu, pol, s_store != 0, gl, sub, lane, acc);
 #endif
 
         warp_fold<NV>(acc);

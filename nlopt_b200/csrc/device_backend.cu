@@ -43,18 +43,26 @@ constexpr int kNumCfgs = (int) (sizeof(kCfgs) / sizeof(kCfgs[0]));
 
 typedef void (*DualKernel)(const DualArgs);
 
-template <int VARIANT, int MAXM, bool FULL, int CFG>
+// measured best geometry per (variant, rows in registers)
+constexpr int default_cfg(int variant, int maxm)
+{
+    return maxm >= 8 ? 3 : maxm == 4 ? (variant == kMMA ? 0 : 1) : (variant == kMMA ? 1 : 2);
+}
+
+template <int VARIANT, int MAXM, bool FULL, int CFG, bool SB = false>
 DualKernel kernel_for(bool store)
 {
     constexpr KernelCfg c = kCfgs[CFG];
-    return store ? (DualKernel) dual_eval_kernel<VARIANT, MAXM, FULL, true, c.block, c.unroll, c.minb>
-                 : (DualKernel) dual_eval_kernel<VARIANT, MAXM, FULL, false, c.block, c.unroll, c.minb>;
+    return store ? (DualKernel) dual_eval_kernel<VARIANT, MAXM, FULL, true, c.block, c.unroll, c.minb, SB>
+                 : (DualKernel) dual_eval_kernel<VARIANT, MAXM, FULL, false, c.block, c.unroll, c.minb, SB>;
 }
 
-// rows kept in registers <= 4: every geometry is built (tuning); 8 or 16 rows need the 128-register budget
+// rows kept in registers <= 4: every geometry is built (tuning); 8 or 16 rows need the 128-register budget.
+// sb (uniform bounds, no lb / ub loads): built for the default geometry only.
 template <int VARIANT, int MAXM, bool FULL>
-DualKernel kernel_by_cfg(int cfg, bool store)
+DualKernel kernel_by_cfg(int cfg, bool store, bool sb)
 {
+    if (sb) return kernel_for<VARIANT, MAXM, FULL, default_cfg(VARIANT, MAXM), true>(store);
     if (MAXM >= 8) return kernel_for<VARIANT, MAXM, FULL, 3>(store);
     switch (cfg) {
     case 1: return kernel_for<VARIANT, (MAXM >= 8 ? 0 : MAXM), FULL, 1>(store);
@@ -65,15 +73,15 @@ DualKernel kernel_by_cfg(int cfg, bool store)
 }
 
 template <int VARIANT, bool FULL>
-DualKernel pick_kernel(int maxm, int cfg, bool store)
+DualKernel pick_kernel(int maxm, int cfg, bool store, bool sb)
 {
     switch (maxm) {
-    case 0: return kernel_by_cfg<VARIANT, 0, FULL>(cfg, store);
-    case 1: return kernel_by_cfg<VARIANT, 1, FULL>(cfg, store);
-    case 2: return kernel_by_cfg<VARIANT, 2, FULL>(cfg, store);
-    case 4: return kernel_by_cfg<VARIANT, 4, FULL>(cfg, store);
-    case 8: return kernel_by_cfg<VARIANT, 8, FULL>(cfg, store);
-    default: return kernel_by_cfg<VARIANT, 16, FULL>(cfg, store);
+    case 0: return kernel_by_cfg<VARIANT, 0, FULL>(cfg, store, sb);
+    case 1: return kernel_by_cfg<VARIANT, 1, FULL>(cfg, store, sb);
+    case 2: return kernel_by_cfg<VARIANT, 2, FULL>(cfg, store, sb);
+    case 4: return kernel_by_cfg<VARIANT, 4, FULL>(cfg, store, sb);
+    case 8: return kernel_by_cfg<VARIANT, 8, FULL>(cfg, store, sb);
+    default: return kernel_by_cfg<VARIANT, 16, FULL>(cfg, store, sb);
     }
 }
 
@@ -94,14 +102,6 @@ DualKernel pick_tma_kernel(int maxm, int stages, bool store)
     case 16: return stages == 2 ? tma_kernel_for<VARIANT, 16, 2, 1>(store) : tma_kernel_for<VARIANT, 16, 2, 1>(store);
     default: return nullptr;
     }
-}
-
-// measured best geometry per (variant, rows in registers)
-int default_cfg(Variant v, int maxm)
-{
-    if (maxm >= 8) return 3;
-    if (maxm == 4) return v == kMMA ? 0 : 1;
-    return v == kMMA ? 1 : 2;
 }
 
 // Process-wide cache of the big allocations (device state pool, pinned staging).  nlopt_optimize
@@ -414,6 +414,9 @@ bool DeviceBackend::setup(const BackendConfig &cfg)
         NB_CUDA(cudaMemcpyAsync(ub_, cfg.ub + j0, nl * sizeof(double), cudaMemcpyHostToDevice, stream_));
         stats_->h2d_bytes += nl * sizeof(double);
     }
+    scalar_bounds_ = cfg.lb_uniform && cfg.ub_uniform;
+    lb_u_ = scalar_bounds_ ? cfg.lb[0] : 0.0;
+    ub_u_ = scalar_bounds_ ? cfg.ub[0] : 0.0;
     bool any_host_cb = cfg.objective.f != nullptr;
     for (const FuncSpec &c : cfg.constraints) any_host_cb = any_host_cb || c.f || c.mf;
     if (cfg.penalty)
@@ -925,6 +928,7 @@ void DeviceBackend::fill_dual_args(DualArgs &a, const double *y, const DualScala
 {
     std::memset(&a, 0, sizeof a);
     a.x = x_; a.lb = lb_; a.ub = ub_; a.sigma = sigma_; a.g = g_; a.G = G_;
+    a.lb_u = lb_u_; a.ub_u = ub_u_;
     a.xcur = xcur_;
     a.ld = geo_.ld;
     a.nchunks = geo_.nchunks; a.chunk0 = geo_.chunk0;
@@ -976,6 +980,13 @@ void DeviceBackend::fill_dual_args(DualArgs &a, const double *y, const DualScala
     a.wide = wide_dev_;
 }
 
+// what `evals` dual evaluations asked HBM for: 3 + m operand arrays with scalar bounds, 5 + m without, + the x* store
+void DeviceBackend::count_operand_bytes(long long evals, bool sb, bool store)
+{
+    const long long per = (long long) (8 * geo_.ld);
+    stats_->dual_operand_bytes += evals * per * ((sb ? 3 : 5) + (long long) m_) + (store ? per : 0);
+}
+
 bool DeviceBackend::launch_dual(const double *y, const DualScalars &sc, bool store, bool wait)
 {
     DualArgs a;
@@ -998,6 +1009,7 @@ bool DeviceBackend::launch_dual(const double *y, const DualScalars &sc, bool sto
     // MMA with 16 gradient rows is register-starved in the register form; the TMA-staged form is the default
     // there.  Everywhere else the register form is faster and the TMA form is opt-in (kernel_cfg 10 / 11 / 12 = 3 / 2 / 4 stages).
     const bool tma_default = kernel_cfg_ < 0 && variant_ == kMMA && maxm == 16 && full_m;
+    bool sb = false;
     if (wide) {
         // any number of constraints: rows streamed in blocks of 8, per-row scalars in dynamic shared memory
         NB_CUDA(cudaMemcpyAsync(wide_dev_, wide_host_.data(), 4 * (size_t) m_ * sizeof(double), cudaMemcpyHostToDevice, stream_));
@@ -1029,9 +1041,10 @@ bool DeviceBackend::launch_dual(const double *y, const DualScalars &sc, bool sto
         // persistent kernel: the grid is sized to the machine, not to the problem (+ the folder CTA)
         int cfg = kernel_cfg_ >= 0 && kernel_cfg_ < kNumCfgs ? kernel_cfg_ : default_cfg(variant_, maxm);
         if (maxm >= 8) cfg = 3;
+        sb = scalar_bounds_ && cfg == default_cfg(variant_, maxm);
         const KernelCfg c = kCfgs[cfg];
-        DualKernel fn = variant_ == kMMA ? (full_m ? pick_kernel<0, true>(maxm, cfg, store) : pick_kernel<0, false>(maxm, cfg, store))
-                                         : (full_m ? pick_kernel<1, true>(maxm, cfg, store) : pick_kernel<1, false>(maxm, cfg, store));
+        DualKernel fn = variant_ == kMMA ? (full_m ? pick_kernel<0, true>(maxm, cfg, store, sb) : pick_kernel<0, false>(maxm, cfg, store, sb))
+                                         : (full_m ? pick_kernel<1, true>(maxm, cfg, store, sb) : pick_kernel<1, false>(maxm, cfg, store, sb));
         const long long want = (long long) geo_.nseg_local;
         const long long cap = (long long) sm_count_ * (ctas_per_sm_ > 0 ? ctas_per_sm_ : 4 * c.minb);
         const int pgrid = (int) (want < cap ? want : cap);
@@ -1040,6 +1053,7 @@ bool DeviceBackend::launch_dual(const double *y, const DualScalars &sc, bool sto
     if (time_kernels_) cudaEventRecord(e1, stream_);
     ++stats_->kernel_launches;
     NB_CUDA(cudaGetLastError());
+    count_operand_bytes(1, sb, store);
     if (!a.publish_host && a.box[0] == nullptr) {
         const int nv = wide ? 3 + (int) m_ : 3 + (maxm > 0 ? maxm : 1);
         if (Comm::instance().all_gather_inplace(out_dev_, (size_t) geo_.local_vshards * nvp_, stream_, &err_)) return false;
@@ -1076,21 +1090,22 @@ typedef void (*SolveKernel)(const SolveArgs);
 #endif
 // `roomy`: the 2-CTAs/SM instantiation (128 registers, no spills in the sweep or in the folder's optimiser turn) -- used
 // when the grid does not need a third CTA per SM anyway (small and mid-size shards), see DeviceBackend::dual_solve
-template <int VARIANT, bool FULL, bool POL>
+// SB: uniform bounds as two scalars (never combined with POL)
+template <int VARIANT, bool FULL, bool POL, bool SB>
 SolveKernel pick_solve_kernel(int maxm, bool roomy)
 {
     if (roomy) switch (maxm) {
-        case 1: return dual_solve_kernel<VARIANT, 1, FULL, POL, 256, 1, 2>;
-        case 2: return dual_solve_kernel<VARIANT, 2, FULL, POL, 256, 1, 2>;
-        case 4: return dual_solve_kernel<VARIANT, 4, FULL, POL, 256, 1, 2>;
+        case 1: return dual_solve_kernel<VARIANT, 1, FULL, POL, 256, 1, 2, SB>;
+        case 2: return dual_solve_kernel<VARIANT, 2, FULL, POL, 256, 1, 2, SB>;
+        case 4: return dual_solve_kernel<VARIANT, 4, FULL, POL, 256, 1, 2, SB>;
         default: break;
         }
     switch (maxm) {
-    case 1: return dual_solve_kernel<VARIANT, 1, FULL, POL, 256, 1, NB200_SOLVE_MINB4>;
-    case 2: return dual_solve_kernel<VARIANT, 2, FULL, POL, 256, 1, NB200_SOLVE_MINB4>;
-    case 4: return dual_solve_kernel<VARIANT, 4, FULL, POL, 256, 1, NB200_SOLVE_MINB4>;
-    case 8: return dual_solve_kernel<VARIANT, 8, FULL, POL, 256, 1, 2>;
-    default: return dual_solve_kernel<VARIANT, 16, FULL, POL, 256, 1, 2>;
+    case 1: return dual_solve_kernel<VARIANT, 1, FULL, POL, 256, 1, NB200_SOLVE_MINB4, SB>;
+    case 2: return dual_solve_kernel<VARIANT, 2, FULL, POL, 256, 1, NB200_SOLVE_MINB4, SB>;
+    case 4: return dual_solve_kernel<VARIANT, 4, FULL, POL, 256, 1, NB200_SOLVE_MINB4, SB>;
+    case 8: return dual_solve_kernel<VARIANT, 8, FULL, POL, 256, 1, 2, SB>;
+    default: return dual_solve_kernel<VARIANT, 16, FULL, POL, 256, 1, 2, SB>;
     }
 }
 // TMA-staged form (full-m, 1 / 2 / 4 rows): {stages, bytes of dynamic shared memory}; 3 CTAs per SM
@@ -1125,11 +1140,16 @@ SolveKernel pick_solve_async_kernel2(int maxm, bool full, int stages)
     return full ? pick_solve_async_kernel<VARIANT, true, 3>(maxm) : pick_solve_async_kernel<VARIANT, false, 3>(maxm);
 }
 
-template <int VARIANT>
-SolveKernel pick_solve_kernel2(int maxm, bool full, bool pol, bool roomy)
+template <int VARIANT, bool FULL>
+SolveKernel pick_solve_kernel1(int maxm, bool pol, bool sb, bool roomy)
 {
-    return full ? (pol ? pick_solve_kernel<VARIANT, true, true>(maxm, roomy) : pick_solve_kernel<VARIANT, true, false>(maxm, roomy))
-                : (pol ? pick_solve_kernel<VARIANT, false, true>(maxm, roomy) : pick_solve_kernel<VARIANT, false, false>(maxm, roomy));
+    if (pol) return pick_solve_kernel<VARIANT, FULL, true, false>(maxm, roomy);
+    return sb ? pick_solve_kernel<VARIANT, FULL, false, true>(maxm, roomy) : pick_solve_kernel<VARIANT, FULL, false, false>(maxm, roomy);
+}
+template <int VARIANT>
+SolveKernel pick_solve_kernel2(int maxm, bool full, bool pol, bool sb, bool roomy)
+{
+    return full ? pick_solve_kernel1<VARIANT, true>(maxm, pol, sb, roomy) : pick_solve_kernel1<VARIANT, false>(maxm, pol, sb, roomy);
 }
 }  // namespace
 
@@ -1188,6 +1208,7 @@ bool DeviceBackend::dual_solve(double *y, const double *lo, const double *hi, co
     size_t smem = 0;
     int block = 256;
     SolveKernel fn = nullptr;
+    bool sb = false;
     if ((solve_tma_ > 0 || tma_auto) && full && !use_pol && (maxm == 1 || maxm == 2 || maxm == 4)) {
         fn = variant_ == kMMA ? pick_solve_tma_kernel<0>(maxm, &smem) : pick_solve_tma_kernel<1>(maxm, &smem);
         block = kTmaBlock;
@@ -1200,7 +1221,8 @@ bool DeviceBackend::dual_solve(double *y, const double *lo, const double *hi, co
     } else {
         // 2 CTAs/SM with 128 registers when that many CTAs already cover the rank's groups (knob b200_solve_minb: 2 / 3 force)
         const bool roomy = solve_minb_ == 2 || (solve_minb_ != 3 && (long long) geo_.nseg_local + 1 <= 2ll * sm_count_);
-        fn = variant_ == kMMA ? pick_solve_kernel2<0>(maxm, full, use_pol, roomy) : pick_solve_kernel2<1>(maxm, full, use_pol, roomy);
+        sb = scalar_bounds_ && !use_pol;
+        fn = variant_ == kMMA ? pick_solve_kernel2<0>(maxm, full, use_pol, sb, roomy) : pick_solve_kernel2<1>(maxm, full, use_pol, sb, roomy);
     }
     int per_sm = 0;
     NB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, block, smem));
@@ -1269,6 +1291,7 @@ bool DeviceBackend::dual_solve(double *y, const double *lo, const double *hi, co
     if (Comm::instance().active() && gens > 0) Comm::instance().advance_seq((unsigned long long) gens);
     if (*ret == kRetInvalid) return true;            // nothing ran; the caller reports it
     if (*ret == kRetFailure) return fail("the cross-rank exchange inside the dual solve timed out");
+    count_operand_bytes(gens, sb, true);             // the last generation stored x*(y)
     out->val = res_host_[0];
     out->gval = res_host_[1];
     out->wval = res_host_[2];

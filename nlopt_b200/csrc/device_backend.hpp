@@ -81,6 +81,7 @@ private:
     void fill_dual_args(struct DualArgs &a, const double *y, const DualScalars &sc);
     bool launch_dual(const double *y, const DualScalars &sc, bool store, bool wait);
     unsigned l2_keep_mask() const;
+    void count_operand_bytes(long long evals, bool sb, bool store);     // nlopt_b200_stats::dual_operand_bytes
     bool wait_flag();
     bool host_x_for(Slot slot);                      // bring the slot's x to pinned host memory (cached per epoch)
     bool push_grad_rows(Slot slot, int row0, unsigned rows, bool is_objective, const double *host_grad);
@@ -115,7 +116,11 @@ private:
     size_t out_rec_ = 0;              // doubles per result record (>= 24, >= 3 + m)
     unsigned long long solve_launch_id_ = 0;   // tag = launch id << 40 | generation: never matches a stale slot
     bool fused_solve_ok_ = true;
-    int kernel_cfg_ = -1;         // -1: measured default for (variant, m)          // index into the launch-geometry table of device_backend.cu
+    // every lb entry is lb_u_ and every ub entry ub_u_ (both set with nlopt_set_*_bounds1): the default dual kernels take
+    // the bounds as two scalars instead of reading the lb / ub arrays, which stay filled for the other kernels
+    bool scalar_bounds_ = false;
+    double lb_u_ = 0.0, ub_u_ = 0.0;
+    int kernel_cfg_ = -1;        // -1: measured default for (variant, m)          // index into the launch-geometry table of device_backend.cu
 
     // device state
     double *pool_ = nullptr;

@@ -1197,6 +1197,7 @@ nlopt_result run_ccsa_precond(nlopt_opt opt, double *x, double *minf, const nb20
             const nlopt_result reti = nlopt_optimize(pre_opt, xcur.data(), &pre_min);
             opt->stats.dual_evals += pre_opt->stats.dual_evals;
             opt->stats.kernel_launches += pre_opt->stats.kernel_launches;
+            opt->stats.dual_operand_bytes += pre_opt->stats.dual_operand_bytes;
             ++opt->stats.dual_solves;
             if (reti < 0 || reti == NLOPT_MAXTIME_REACHED) {
                 if (reti < 0 && nlopt_get_errmsg(pre_opt)) set_err(opt, "nested model solve: %s", nlopt_get_errmsg(pre_opt));
