@@ -1993,6 +1993,8 @@ __global__ void __launch_bounds__(kBlock, MINB) dual_solve_async_kernel(const __
 //     tagged slots.  Same lanes, same per-warp accumulators, same fold tree: the same bits as every other kernel here.
 //   leaving: when the solve is over the consumers stop the producer and wait for the copies it has already issued
 //     (a CTA must not retire with bulk copies into its shared memory in flight).
+// SB (uniform bounds, as in sweep_group): a stage holds 3 + m arrays {x, sigma, g, G_0..}; no lb / ub copies are issued
+// and the consumers hand make_double2(lb_u, lb_u) / make_double2(ub_u, ub_u) to the unchanged closed forms.
 struct StageMeta {
     unsigned long long gen;       // generation the chunk belongs to
     unsigned long long p;         // pair offset of the chunk
@@ -2008,12 +2010,13 @@ __device__ __forceinline__ bool mbar_test(unsigned long long *bar, unsigned pari
     return ok != 0;
 }
 
-template <int VARIANT, int MAXM, int STAGES, int MINB>
+template <int VARIANT, int MAXM, int STAGES, int MINB, bool SB>
 __global__ void __launch_bounds__(kTmaBlock, MINB) dual_solve_tma_kernel(const __grid_constant__ SolveArgs sa)
 {
     constexpr int MR = MAXM > 0 ? MAXM : 1;
     constexpr int NV = 3 + MR;
-    constexpr int NARR = 5 + MAXM;
+    constexpr int NB = SB ? 0 : 2;                            // bound arrays in a stage
+    constexpr int NARR = 3 + NB + MAXM;
     static_assert(MAXM >= 1, "the solve kernels need at least one constraint");
     extern __shared__ __align__(128) unsigned char s_raw[];
     double2 *s_tile = reinterpret_cast<double2 *>(s_raw);     // [STAGES][NARR][kChunkPairs]
@@ -2054,9 +2057,11 @@ __global__ void __launch_bounds__(kTmaBlock, MINB) dual_solve_tma_kernel(const _
         // ---------------- producer ----------------
         if (lane == 0) {
             const double *src[NARR];
-            src[0] = a.x; src[1] = a.lb; src[2] = a.ub; src[3] = a.sigma; src[4] = a.g;
+            src[0] = a.x;
+            if (!SB) { src[1] = a.lb; src[2] = a.ub; }
+            src[1 + NB] = a.sigma; src[2 + NB] = a.g;
 #pragma unroll
-            for (int i = 0; i < MAXM; ++i) src[5 + i] = a.G + (unsigned long long) i * a.ld;
+            for (int i = 0; i < MAXM; ++i) src[3 + NB + i] = a.G + (unsigned long long) i * a.ld;
             int st = 0;
             unsigned phase = 0;
             unsigned long long issued = 0;
@@ -2150,9 +2155,17 @@ __global__ void __launch_bounds__(kTmaBlock, MINB) dual_solve_tma_kernel(const _
         const bool has = !(mt.flags & 4u);
         if (has) {
             const double2 *t = s_tile + (size_t) st * NARR * kChunkPairs + sub * 32 + lane;
-            vx = t[0]; vlb = t[kChunkPairs]; vub = t[2 * kChunkPairs]; vs = t[3 * kChunkPairs]; vg = t[4 * kChunkPairs];
+            vx = t[0];
+            if (SB) {
+                vlb = make_double2(a.lb_u, a.lb_u);
+                vub = make_double2(a.ub_u, a.ub_u);
+            } else {
+                vlb = t[kChunkPairs];
+                vub = t[2 * kChunkPairs];
+            }
+            vs = t[(1 + NB) * kChunkPairs]; vg = t[(2 + NB) * kChunkPairs];
 #pragma unroll
-            for (int i = 0; i < MAXM; ++i) { const double2 g2 = t[(5 + i) * kChunkPairs]; Ga[i] = g2.x; Gb[i] = g2.y; }
+            for (int i = 0; i < MAXM; ++i) { const double2 g2 = t[(3 + NB + i) * kChunkPairs]; Ga[i] = g2.x; Gb[i] = g2.y; }
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(&s_empty[st]);             // operands are in registers: release the stage

@@ -1108,14 +1108,20 @@ SolveKernel pick_solve_kernel(int maxm, bool roomy)
     default: return dual_solve_kernel<VARIANT, 16, FULL, POL, 256, 1, 2, SB>;
     }
 }
-// TMA-staged form (full-m, 1 / 2 / 4 rows): {stages, bytes of dynamic shared memory}; 3 CTAs per SM
-template <int VARIANT>
+// TMA-staged form (full-m, 1 / 2 / 4 rows): {stages, bytes of dynamic shared memory}.  A stage is (5 + m) x 4 KB,
+// (3 + m) x 4 KB with uniform bounds (SB).  3 CTAs per SM, except SB with 4 rows: 3 stages of 28 KB at 2 CTAs/SM
+// (96 registers, no spills for CCSAQ) -- on the H100 at n = 1e7 198-206 us per evaluation against 236-241 us for
+// 2 stages at 3 CTAs/SM (72 registers, 88 B of spills), DESIGN.md section 3.2.
+template <int VARIANT, bool SB>
 SolveKernel pick_solve_tma_kernel(int maxm, size_t *smem)
 {
+    constexpr size_t nb = SB ? 3 : 5;
     switch (maxm) {
-    case 1: *smem = (size_t) 3 * 6 * kChunkBytes; return dual_solve_tma_kernel<VARIANT, 1, 3, 3>;
-    case 2: *smem = (size_t) 2 * 7 * kChunkBytes; return dual_solve_tma_kernel<VARIANT, 2, 2, 3>;
-    case 4: *smem = (size_t) 2 * 9 * kChunkBytes; return dual_solve_tma_kernel<VARIANT, 4, 2, 3>;
+    case 1: *smem = 3 * (nb + 1) * kChunkBytes; return dual_solve_tma_kernel<VARIANT, 1, 3, 3, SB>;
+    case 2: *smem = 2 * (nb + 2) * kChunkBytes; return dual_solve_tma_kernel<VARIANT, 2, 2, 3, SB>;
+    case 4:
+        if (SB) { *smem = 3 * (nb + 4) * kChunkBytes; return dual_solve_tma_kernel<VARIANT, 4, 3, 2, SB>; }
+        *smem = 2 * (nb + 4) * kChunkBytes; return dual_solve_tma_kernel<VARIANT, 4, 2, 3, SB>;
     default: *smem = 0; return nullptr;
     }
 }
@@ -1200,17 +1206,21 @@ bool DeviceBackend::dual_solve(double *y, const double *lo, const double *hi, co
     const int maxm = pick_maxm((int) m_);
     const bool full = (int) m_ == maxm && (variant_ == kCCSAQ || sa.d.active == ((1u << m_) - 1u));
     const bool use_pol = sa.d.l2_keep != 0u;
-    // Small shards are latency-bound in the register form (a CTA walks a handful of chunks, one dependent load ->
-    // compute step each): there the TMA-staged form, whose producer warp runs ahead across generations, is the default
-    // (knob b200_solve_tma: 1 always, 0 never).  Large shards are HBM-bound in the register form.
-    const size_t operand_bytes = (5 + (size_t) m_) * geo_.ld * sizeof(double);
-    const bool tma_auto = solve_tma_ < 0 && operand_bytes <= ((size_t) 400 << 20);
+    // With uniform bounds the TMA-staged form, whose producer warp keeps the next chunks in flight during the arithmetic
+    // and across group and generation boundaries, is the default for 4 rows at every size measured (n = 1.25e6 .. 5e7,
+    // MMA and CCSAQ) and for 1 row up to 80 MB of operands (n <= 2.5e6); above that the two forms tie with 1 row, and
+    // CCSAQ lost 8 % at n = 5e7.  2 rows (not measured), bound arrays and L2 policies keep the register form
+    // (DESIGN.md section 3.2; knob b200_solve_tma: 1 always, 0 never).
+    const size_t operand_bytes = (3 + (size_t) m_) * geo_.ld * sizeof(double);
+    const bool tma_auto = solve_tma_ < 0 && scalar_bounds_ && (maxm == 4 || (maxm == 1 && operand_bytes <= ((size_t) 80 << 20)));
     size_t smem = 0;
     int block = 256;
     SolveKernel fn = nullptr;
     bool sb = false;
     if ((solve_tma_ > 0 || tma_auto) && full && !use_pol && (maxm == 1 || maxm == 2 || maxm == 4)) {
-        fn = variant_ == kMMA ? pick_solve_tma_kernel<0>(maxm, &smem) : pick_solve_tma_kernel<1>(maxm, &smem);
+        sb = scalar_bounds_;
+        fn = variant_ == kMMA ? (sb ? pick_solve_tma_kernel<0, true>(maxm, &smem) : pick_solve_tma_kernel<0, false>(maxm, &smem))
+                              : (sb ? pick_solve_tma_kernel<1, true>(maxm, &smem) : pick_solve_tma_kernel<1, false>(maxm, &smem));
         block = kTmaBlock;
         NB_CUDA(cudaFuncSetAttribute((const void *) fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
     } else if (solve_async_ >= 2 && !use_pol && maxm <= 8) {

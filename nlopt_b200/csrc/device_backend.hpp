@@ -106,7 +106,7 @@ private:
     double *wide_dev_ = nullptr;      // m > 16: y | rhoc | rhoc/2 | active flags of the evaluation in flight
     std::vector<double> wide_host_;
     size_t l2_keep_bytes_ = 0;        // operand bytes to load evict_last (knob b200_l2_keep_mb)
-    int solve_tma_ = 0;               // knob b200_solve_tma: 0 register form (default: faster at every size measured), 1 TMA-staged form, -1 by size
+    int solve_tma_ = -1;              // knob b200_solve_tma: -1 by rows, bounds and size (DeviceBackend::dual_solve), 0 register form, 1 TMA-staged form
     int solve_async_ = NB200_SOLVE_ASYNC_DEFAULT;   // knob b200_solve_async: 0 register form, 2 / 3: per-thread cp.async operand ring of 2 / 3 stages
     int solve_minb_ = 0;              // knob b200_solve_minb: 0 by size, 2 / 3: force the 2- / 3-CTAs-per-SM instantiation of the solve kernel
     unsigned stagger_ns_ = NB200_STAGGER_NS_DEFAULT;   // knob b200_stagger_ns: start-of-generation skew between warps sharing an SM sub-partition
