@@ -60,6 +60,9 @@ inline Workspace &workspace()
         cudaMemset(w.ticket, 0, sizeof(unsigned));
         cudaMalloc(&w.result_dev, sizeof(double));
         cudaHostAlloc(&w.result_host, sizeof(double), cudaHostAllocDefault);
+        // the memset runs on the legacy default stream, which does not order work on a non-blocking stream (the
+        // library's): let it complete before the first map_reduce_kernel reads the ticket
+        cudaDeviceSynchronize();
     }
     return w;
 }
