@@ -271,7 +271,12 @@ typedef struct {
     long long dual_operand_bytes; /* HBM bytes the dual kernels were asked to read on this rank, summed over evaluations,
                                      plus their stores of x*(y): 8 ld (3 + m) per evaluation when both bounds are
                                      uniform (nlopt_set_*_bounds1) and the default kernels run, 8 ld (5 + m) otherwise;
-                                     ld = this rank's padded shard length */
+                                     ld = this rank's padded shard length; with the sigma index (below) the default
+                                     TMA-staged solve kernel reads 8 ld (2 + m) + 2 ld instead of 8 ld (3 + m) */
+    long long sigma_palette;     /* entries of the sigma palette at the end of the run, 0 when the dual kernels no
+                                     longer read sigma as a 16-bit index into it (bounds or initial step not uniform,
+                                     palette past its 65535-entry cap, or a self-check mismatch)                   */
+    long long sigma_index_mismatches;  /* variables whose updated sigma differed from its palette entry (expected 0)  */
 } nlopt_b200_stats;
 nlopt_result nlopt_b200_get_stats(const nlopt_opt opt, nlopt_b200_stats *out);
 

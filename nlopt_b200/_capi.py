@@ -35,6 +35,7 @@ class Stats(C.Structure):
         ("h2d_bytes", C.c_longlong), ("d2h_bytes", C.c_longlong), ("kernel_launches", C.c_longlong),
         ("seconds_setup", C.c_double), ("seconds_dual_wall", C.c_double), ("seconds_eval_wall", C.c_double),
         ("seconds_glue_wall", C.c_double), ("dual_operand_bytes", C.c_longlong),
+        ("sigma_palette", C.c_longlong), ("sigma_index_mismatches", C.c_longlong),
     ]
 
 

@@ -277,6 +277,10 @@ struct DualArgs {
     double y[kMaxParamM], rhoc[kMaxParamM], half_rhoc[kMaxParamM];       // (m <= 16)
     const double *wide;           // m > 16: device block  y[m] | rhoc[m] | half_rhoc[m] | active[m] (1.0 / 0.0)
     double lb_u, ub_u;            // the value of every lb / ub entry when both are uniform (read by the SB instantiations)
+    // sigma index (DeviceBackend: valid with uniform bounds and a uniform initial step): sigma[j] == pal[sidx[j]] bit for
+    // bit, read by the kSigmaIndex instantiations of dual_solve_tma_kernel instead of sigma
+    const unsigned short *sidx;
+    const double *pal;
     __device__ __forceinline__ double u() const { return u_ccsaq; }
 };
 
@@ -1993,8 +1997,15 @@ __global__ void __launch_bounds__(kBlock, MINB) dual_solve_async_kernel(const __
 //     tagged slots.  Same lanes, same per-warp accumulators, same fold tree: the same bits as every other kernel here.
 //   leaving: when the solve is over the consumers stop the producer and wait for the copies it has already issued
 //     (a CTA must not retire with bulk copies into its shared memory in flight).
-// SB (uniform bounds, as in sweep_group): a stage holds 3 + m arrays {x, sigma, g, G_0..}; no lb / ub copies are issued
-// and the consumers hand make_double2(lb_u, lb_u) / make_double2(ub_u, ub_u) to the unchanged closed forms.
+// BM, which operands a stage holds:
+//   kBoundArrays:  5 + m arrays {x, lb, ub, sigma, g, G_0..}
+//   kScalarBounds (uniform bounds, as SB in sweep_group): 3 + m arrays {x, sigma, g, G_0..}; no lb / ub copies are issued
+//     and the consumers hand make_double2(lb_u, lb_u) / make_double2(ub_u, ub_u) to the unchanged closed forms
+//   kSigmaIndex (uniform bounds and the sigma index is valid, sigma_palette.hpp): 2 + m arrays {x, g, G_0..} and the
+//     chunk's 512 16-bit sigma indices (1 KB); the consumers look sigma up in the palette and hand the closed forms the
+//     same double2 as the fp64 array would have given.
+enum : int { kBoundArrays = 0, kScalarBounds = 1, kSigmaIndex = 2 };
+constexpr unsigned kIdxChunkBytes = 2 * 2 * kChunkPairs;
 struct StageMeta {
     unsigned long long gen;       // generation the chunk belongs to
     unsigned long long p;         // pair offset of the chunk
@@ -2010,16 +2021,19 @@ __device__ __forceinline__ bool mbar_test(unsigned long long *bar, unsigned pari
     return ok != 0;
 }
 
-template <int VARIANT, int MAXM, int STAGES, int MINB, bool SB>
+template <int VARIANT, int MAXM, int STAGES, int MINB, int BM>
 __global__ void __launch_bounds__(kTmaBlock, MINB) dual_solve_tma_kernel(const __grid_constant__ SolveArgs sa)
 {
     constexpr int MR = MAXM > 0 ? MAXM : 1;
     constexpr int NV = 3 + MR;
-    constexpr int NB = SB ? 0 : 2;                            // bound arrays in a stage
-    constexpr int NARR = 3 + NB + MAXM;
+    constexpr int NB = BM == kBoundArrays ? 2 : 0;           // bound arrays in a stage
+    constexpr bool SIDX = BM == kSigmaIndex;
+    constexpr int KG = SIDX ? 1 + NB : 2 + NB;                // tile of grad f; sigma (fp64) is tile 1 + NB
+    constexpr int NARR = KG + 1 + MAXM;                       // fp64 tiles in a stage
     static_assert(MAXM >= 1, "the solve kernels need at least one constraint");
     extern __shared__ __align__(128) unsigned char s_raw[];
     double2 *s_tile = reinterpret_cast<double2 *>(s_raw);     // [STAGES][NARR][kChunkPairs]
+    const unsigned *s_idx = reinterpret_cast<const unsigned *>(s_raw + (size_t) STAGES * NARR * kChunkBytes);   // [STAGES][kChunkPairs] (SIDX)
     __shared__ unsigned long long s_full[STAGES], s_empty[STAGES];
     __shared__ StageMeta s_meta[STAGES];
     __shared__ double s_rec[2][kGroupWarps * NV];
@@ -2058,10 +2072,11 @@ __global__ void __launch_bounds__(kTmaBlock, MINB) dual_solve_tma_kernel(const _
         if (lane == 0) {
             const double *src[NARR];
             src[0] = a.x;
-            if (!SB) { src[1] = a.lb; src[2] = a.ub; }
-            src[1 + NB] = a.sigma; src[2 + NB] = a.g;
+            if (NB) { src[1] = a.lb; src[2] = a.ub; }
+            if (!SIDX) src[1 + NB] = a.sigma;
+            src[KG] = a.g;
 #pragma unroll
-            for (int i = 0; i < MAXM; ++i) src[3 + NB + i] = a.G + (unsigned long long) i * a.ld;
+            for (int i = 0; i < MAXM; ++i) src[KG + 1 + i] = a.G + (unsigned long long) i * a.ld;
             int st = 0;
             unsigned phase = 0;
             unsigned long long issued = 0;
@@ -2084,10 +2099,12 @@ __global__ void __launch_bounds__(kTmaBlock, MINB) dual_solve_tma_kernel(const _
                     if (empty) {
                         mbar_arrive(&s_full[st]);                         // no bytes: the phase completes on this arrival
                     } else {
-                        mbar_expect_tx(&s_full[st], NARR * kChunkBytes);
+                        mbar_expect_tx(&s_full[st], NARR * kChunkBytes + (SIDX ? kIdxChunkBytes : 0u));
 #pragma unroll
                         for (int k = 0; k < NARR; ++k)
                             tma_bulk_load(s_tile + ((size_t) st * NARR + k) * kChunkPairs, src[k] + 2 * p, kChunkBytes, &s_full[st]);
+                        if (SIDX)
+                            tma_bulk_load((void *) (s_idx + (size_t) st * kChunkPairs), a.sidx + 2 * p, kIdxChunkBytes, &s_full[st]);
                     }
                     s_issued = ++issued;
                     if (++st == STAGES) { st = 0; phase ^= 1u; }
@@ -2153,24 +2170,28 @@ __global__ void __launch_bounds__(kTmaBlock, MINB) dual_solve_tma_kernel(const _
 #pragma unroll
         for (int i = 0; i < MR; ++i) { Ga[i] = 0.0; Gb[i] = 0.0; }
         const bool has = !(mt.flags & 4u);
+        unsigned iw = 0;                                      // SIDX: the two 16-bit sigma indices of this lane's pair
         if (has) {
             const double2 *t = s_tile + (size_t) st * NARR * kChunkPairs + sub * 32 + lane;
             vx = t[0];
-            if (SB) {
-                vlb = make_double2(a.lb_u, a.lb_u);
-                vub = make_double2(a.ub_u, a.ub_u);
-            } else {
+            if (NB) {
                 vlb = t[kChunkPairs];
                 vub = t[2 * kChunkPairs];
+            } else {
+                vlb = make_double2(a.lb_u, a.lb_u);
+                vub = make_double2(a.ub_u, a.ub_u);
             }
-            vs = t[(1 + NB) * kChunkPairs]; vg = t[(2 + NB) * kChunkPairs];
+            if (SIDX) iw = s_idx[(size_t) st * kChunkPairs + sub * 32 + lane];
+            else vs = t[(1 + NB) * kChunkPairs];
+            vg = t[KG * kChunkPairs];
 #pragma unroll
-            for (int i = 0; i < MAXM; ++i) { const double2 g2 = t[(3 + NB + i) * kChunkPairs]; Ga[i] = g2.x; Gb[i] = g2.y; }
+            for (int i = 0; i < MAXM; ++i) { const double2 g2 = t[(KG + 1 + i) * kChunkPairs]; Ga[i] = g2.x; Gb[i] = g2.y; }
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(&s_empty[st]);             // operands are in registers: release the stage
         if (++st == STAGES) { st = 0; phase ^= 1u; }
         ++consumed;
+        if (SIDX && has) vs = make_double2(__ldg(a.pal + (iw & 0xffffu)), __ldg(a.pal + (iw >> 16)));
         if (has) {
             double2 xc;
             if (VARIANT == 0) {
@@ -2302,8 +2323,9 @@ __global__ void fill_kernel(double *dst, double value, unsigned long long n_loca
 // ---- sigma initialisation, mma.c:202-210 ---------------------------------------------------------
 __device__ __forceinline__ bool dev_isinf(double v) { return fabs(v) >= HUGE_VAL * 0.99 || isinf(v); }
 
+// sidx (or null): the sigma index, whose palette entry 1 is the one value this kernel writes (sigma_palette.hpp)
 __global__ void sigma_init_kernel(double *sigma, const double *lb, const double *ub, const double *sigma_init,
-                                  double sigma_min, unsigned long long n_local)
+                                  double sigma_min, unsigned long long n_local, unsigned short *sidx)
 {
     for (unsigned long long j = blockIdx.x * (unsigned long long) blockDim.x + threadIdx.x; j < n_local;
          j += (unsigned long long) gridDim.x * blockDim.x) {
@@ -2312,6 +2334,7 @@ __global__ void sigma_init_kernel(double *sigma, const double *lb, const double 
         else if (dev_isinf(ub[j]) || dev_isinf(lb[j])) s = 1.0;
         else s = mulx(0.5, subx(ub[j], lb[j]));
         sigma[j] = s > sigma_min ? s : sigma_min;
+        if (sidx) sidx[j] = 1;
     }
 }
 
@@ -2334,17 +2357,22 @@ struct EndOuterArgs {
     int update_sigma;         // k > 1
     double kappa;             // 0.01 (mma.c:439) or 1e-8 (ccsa_quadratic.c:587)
     double sigma_min;
+    // sigma index (or null sidx): sidx[j] <- next[3 sidx[j] + branch]; every variable whose new sigma differs from
+    // pal[sidx[j]] is counted into the 4th sum, and the host stops using the index
+    unsigned short *sidx;
+    const unsigned short *next;
+    const double *pal;
 };
 
 __global__ void __launch_bounds__(kBlock) end_outer_kernel(const __grid_constant__ EndOuterArgs a)
 {
-    constexpr int NV = 3;     // sum w|dx|, sum w|x|, count of |dx| >= xtol_abs
+    constexpr int NV = 4;     // sum w|dx|, sum w|x|, count of |dx| >= xtol_abs, count of sigma index mismatches
     __shared__ double s_red[kWarps * NV];
     __shared__ int s_flag;
     const unsigned seg = a.seg0 + blockIdx.x;
     unsigned long long p_lo, p_hi;
     group_pairs(a.nchunks, a.nseg_total, a.chunk0, seg, &p_lo, &p_hi);
-    double acc[NV] = {0.0, 0.0, 0.0};
+    double acc[NV] = {0.0, 0.0, 0.0, 0.0};
     for (unsigned long long p = p_lo + threadIdx.x; p < p_hi; p += kBlock) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -2363,7 +2391,9 @@ __global__ void __launch_bounds__(kBlock) end_outer_kernel(const __grid_constant
             if (a.update_sigma) {
                 const double xpp = a.xprevprev[j];
                 const double osc = mulx(subx(xc, xp), subx(xp, xpp));
-                double s = mulx(a.sigma[j], osc < 0 ? 0.7 : (osc > 0 ? 1.2 : 1.0));
+                const int br = osc < 0 ? 0 : (osc > 0 ? 1 : 2);
+                const double s0 = a.sigma[j];
+                double s = mulx(s0, br == 0 ? 0.7 : (br == 1 ? 1.2 : 1.0));
                 const double lo = a.lb[j], hi = a.ub[j];
                 if (!dev_isinf(hi) && !dev_isinf(lo)) {
                     const double range = subx(hi, lo);
@@ -2371,7 +2401,15 @@ __global__ void __launch_bounds__(kBlock) end_outer_kernel(const __grid_constant
                     s = s < top ? s : top;
                     s = s > bot ? s : bot;
                 }
-                a.sigma[j] = s > a.sigma_min ? s : a.sigma_min;
+                s = s > a.sigma_min ? s : a.sigma_min;
+                a.sigma[j] = s;
+                if (a.sidx) {     // the index before the update (sigma_0 included) and after it must both match
+                    const unsigned short i0 = a.sidx[j], t = a.next[3u * i0 + br];
+                    a.sidx[j] = t;
+                    if (__double_as_longlong(__ldg(a.pal + i0)) != __double_as_longlong(s0) ||
+                        __double_as_longlong(__ldg(a.pal + t)) != __double_as_longlong(s))
+                        acc[3] = addx(acc[3], 1.0);
+                }
             }
             a.xprevprev[j] = xp;
             a.xprev[j] = xc;
@@ -2380,7 +2418,7 @@ __global__ void __launch_bounds__(kBlock) end_outer_kernel(const __grid_constant
     block_reduce_to<NV>(acc, s_red, a.partials + (unsigned long long) blockIdx.x * a.nvp);
     const unsigned vs_local = blockIdx.x / a.segs_per_vshard;
     if (!is_last_arrival(a.tickets + vs_local, a.segs_per_vshard, &s_flag)) return;
-    acc[0] = acc[1] = acc[2] = 0.0;
+    acc[0] = acc[1] = acc[2] = acc[3] = 0.0;
     {
         const double *base = a.partials + (unsigned long long) vs_local * a.segs_per_vshard * a.nvp;
         for (unsigned sgi = threadIdx.x; sgi < a.segs_per_vshard; sgi += kBlock)

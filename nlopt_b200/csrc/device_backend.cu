@@ -178,7 +178,7 @@ cudaError_t cached_host_alloc(double **p, size_t bytes)
     return cudaHostAlloc(p, bytes, cudaHostAllocMapped);
 }
 
-constexpr int kEndNvp = 4;          // end_outer_kernel: record stride (3 sums)
+constexpr int kEndNvp = 4;          // end_outer_kernel: record stride (4 sums)
 constexpr size_t kGuard = 8;        // doubles of guard around x and xcur (halo cells)
 
 int pick_maxm(int m) { return m == 0 ? 0 : m <= 1 ? 1 : m <= 2 ? 2 : m <= 4 ? 4 : m <= 8 ? 8 : 16; }
@@ -335,7 +335,7 @@ bool DeviceBackend::alloc_workspace()
     }
     const size_t ng = geo_.nseg_local;
     const size_t rec = (size_t) (nvp_ > 24 ? nvp_ : 24);
-    if (!small_dev((void **) &partials_, ng * kEndNvp * sizeof(double))) return false;   // end_outer_kernel: one record (3 sums, stride 4) per group
+    if (!small_dev((void **) &partials_, ng * kEndNvp * sizeof(double))) return false;   // end_outer_kernel: one record (4 sums) per group
     // tagged group records {value, tag} of the dual kernels: [nvp][local groups]; tags never repeat (launch ids), so
     // the slots only have to start from zero once
     {
@@ -417,6 +417,15 @@ bool DeviceBackend::setup(const BackendConfig &cfg)
     scalar_bounds_ = cfg.lb_uniform && cfg.ub_uniform;
     lb_u_ = scalar_bounds_ ? cfg.lb[0] : 0.0;
     ub_u_ = scalar_bounds_ ? cfg.ub[0] : 0.0;
+    sidx_valid_ = false;
+    if (scalar_bounds_ && m_ == 4) {          // the sigma index and its palette (device + pinned staging), sized for the cap once
+        if (!small_dev((void **) &sidx_, geo_.ld * sizeof(unsigned short))) return false;
+        if (!small_dev((void **) &pal_, SigmaPalette::kCap * sizeof(double))) return false;
+        if (!small_dev((void **) &next_, SigmaPalette::kCap * 3 * sizeof(unsigned short))) return false;
+        if (!small_pinned((void **) &pal_pinned_, SigmaPalette::kCap * sizeof(double))) return false;
+        if (!small_pinned((void **) &next_pinned_, SigmaPalette::kCap * 3 * sizeof(unsigned short))) return false;
+        NB_CUDA(cudaMemsetAsync(sidx_, 0, geo_.ld * sizeof(unsigned short), stream_));
+    }
     bool any_host_cb = cfg.objective.f != nullptr;
     for (const FuncSpec &c : cfg.constraints) any_host_cb = any_host_cb || c.f || c.mf;
     if (cfg.penalty)
@@ -488,13 +497,60 @@ bool DeviceBackend::sigma_init_from(const double *sigma_init_host, double sigma_
         stats_->h2d_bytes += nl * sizeof(double);
         init_dev = xprevprev_;
     }
-    sigma_init_kernel<<<grid_for(nl, sm_count_), kBlock, 0, stream_>>>(sigma_, lb_, ub_, init_dev, sigma_min, nl);
+    // the sigma index needs one sigma_0: uniform bounds, and no initial step or the same one for every variable (all of
+    // them, so that every rank decides alike); it is kept only when the solve kernel that reads it will run
+    sidx_valid_ = sidx_ != nullptr && sigma_index_runs();
+    if (sidx_valid_ && sigma_init_host)
+        for (size_t j = 1; j < (size_t) geo_.n && sidx_valid_; ++j)
+            sidx_valid_ = std::memcmp(sigma_init_host + j, sigma_init_host, sizeof(double)) == 0;
+    if (sidx_valid_) {
+        palette_.reset(SigmaPalette::sigma0(lb_u_, ub_u_, sigma_init_host ? sigma_init_host[0] : 0.0, sigma_min), lb_u_, ub_u_,
+                       variant_ == kMMA ? 0.01 : 1e-8, sigma_min);
+        sidx_sigma_min_ = sigma_min;
+        pal_uploaded_ = rows_uploaded_ = 0;
+        if (!upload_palette()) return false;
+    }
+    stats_->sigma_palette = sidx_valid_ ? (long long) palette_.val.size() : 0;
+    sigma_init_kernel<<<grid_for(nl, sm_count_), kBlock, 0, stream_>>>(sigma_, lb_, ub_, init_dev, sigma_min, nl,
+                                                                        sidx_valid_ ? sidx_ : nullptr);
     ++stats_->kernel_launches;
     NB_CUDA(cudaGetLastError());
     return true;
 }
 
 bool DeviceBackend::init_sigma(double sigma_min) { return sigma_init_from(cfg_.sigma_init, sigma_min); }
+
+// The sigma-index form of the TMA-staged solve kernel runs -- and only then is the index kept -- with uniform bounds,
+// 4 rows, the TMA form chosen by the default rule (knob b200_solve_tma = 1 forces the TMA form with the fp64 sigma),
+// no L2 policy, the fused solve, and an fp64 operand set of more than NB200_SIGMA_INDEX_MIN_MB (DESIGN.md section 3.2:
+// below it the palette lookup is not paid back).
+bool DeviceBackend::sigma_index_runs() const
+{
+    const size_t operand_bytes = (3 + (size_t) m_) * geo_.ld * sizeof(double);
+    return scalar_bounds_ && m_ == 4 && solve_tma_ < 0 && l2_keep_bytes_ == 0 && supports_dual_solve() &&
+           operand_bytes > ((size_t) NB200_SIGMA_INDEX_MIN_MB << 20);
+}
+
+// the palette entries and transition rows added since the last upload, through pinned staging on the library stream
+// (entries are append-only: a slot of the staging is never rewritten while its copy may be in flight)
+bool DeviceBackend::upload_palette()
+{
+    const size_t nv = palette_.val.size(), nr = palette_.rows();
+    if (nv > pal_uploaded_) {
+        std::memcpy(pal_pinned_ + pal_uploaded_, palette_.val.data() + pal_uploaded_, (nv - pal_uploaded_) * sizeof(double));
+        NB_CUDA(cudaMemcpyAsync(pal_ + pal_uploaded_, pal_pinned_ + pal_uploaded_, (nv - pal_uploaded_) * sizeof(double),
+                                cudaMemcpyHostToDevice, stream_));
+    }
+    if (nr > rows_uploaded_) {
+        std::memcpy(next_pinned_ + 3 * rows_uploaded_, palette_.next.data() + 3 * rows_uploaded_,
+                    3 * (nr - rows_uploaded_) * sizeof(unsigned short));
+        NB_CUDA(cudaMemcpyAsync(next_ + 3 * rows_uploaded_, next_pinned_ + 3 * rows_uploaded_,
+                                3 * (nr - rows_uploaded_) * sizeof(unsigned short), cudaMemcpyHostToDevice, stream_));
+    }
+    pal_uploaded_ = nv;
+    rows_uploaded_ = nr;
+    return true;
+}
 
 // ------------------------------------------------------------------------------------------------
 // user functions
@@ -929,6 +985,7 @@ void DeviceBackend::fill_dual_args(DualArgs &a, const double *y, const DualScala
     std::memset(&a, 0, sizeof a);
     a.x = x_; a.lb = lb_; a.ub = ub_; a.sigma = sigma_; a.g = g_; a.G = G_;
     a.lb_u = lb_u_; a.ub_u = ub_u_;
+    a.sidx = sidx_valid_ ? sidx_ : nullptr; a.pal = pal_;
     a.xcur = xcur_;
     a.ld = geo_.ld;
     a.nchunks = geo_.nchunks; a.chunk0 = geo_.chunk0;
@@ -980,11 +1037,12 @@ void DeviceBackend::fill_dual_args(DualArgs &a, const double *y, const DualScala
     a.wide = wide_dev_;
 }
 
-// what `evals` dual evaluations asked HBM for: 3 + m operand arrays with scalar bounds, 5 + m without, + the x* store
-void DeviceBackend::count_operand_bytes(long long evals, bool sb, bool store)
+// what `evals` dual evaluations asked HBM for: 3 + m operand arrays with scalar bounds, 5 + m without, + the x* store;
+// with the sigma index (si) 2 bytes per variable replace the sigma array
+void DeviceBackend::count_operand_bytes(long long evals, bool sb, bool si, bool store)
 {
     const long long per = (long long) (8 * geo_.ld);
-    stats_->dual_operand_bytes += evals * per * ((sb ? 3 : 5) + (long long) m_) + (store ? per : 0);
+    stats_->dual_operand_bytes += evals * (per * ((sb ? 3 : 5) - (si ? 1 : 0) + (long long) m_) + (si ? per / 4 : 0)) + (store ? per : 0);
 }
 
 bool DeviceBackend::launch_dual(const double *y, const DualScalars &sc, bool store, bool wait)
@@ -1053,7 +1111,7 @@ bool DeviceBackend::launch_dual(const double *y, const DualScalars &sc, bool sto
     if (time_kernels_) cudaEventRecord(e1, stream_);
     ++stats_->kernel_launches;
     NB_CUDA(cudaGetLastError());
-    count_operand_bytes(1, sb, store);
+    count_operand_bytes(1, sb, false, store);
     if (!a.publish_host && a.box[0] == nullptr) {
         const int nv = wide ? 3 + (int) m_ : 3 + (maxm > 0 ? maxm : 1);
         if (Comm::instance().all_gather_inplace(out_dev_, (size_t) geo_.local_vshards * nvp_, stream_, &err_)) return false;
@@ -1109,21 +1167,37 @@ SolveKernel pick_solve_kernel(int maxm, bool roomy)
     }
 }
 // TMA-staged form (full-m, 1 / 2 / 4 rows): {stages, bytes of dynamic shared memory}.  A stage is (5 + m) x 4 KB,
-// (3 + m) x 4 KB with uniform bounds (SB).  3 CTAs per SM, except SB with 4 rows: 3 stages of 28 KB at 2 CTAs/SM
+// (3 + m) x 4 KB with uniform bounds (kScalarBounds), (2 + m) x 4 KB + 1 KB with the sigma index (kSigmaIndex).
+// 3 CTAs per SM, except 4 rows with uniform bounds: 3 stages of 28 KB (25 KB with the sigma index) at 2 CTAs/SM
 // (96 registers, no spills for CCSAQ) -- on the H100 at n = 1e7 198-206 us per evaluation against 236-241 us for
 // 2 stages at 3 CTAs/SM (72 registers, 88 B of spills), DESIGN.md section 3.2.
-template <int VARIANT, bool SB>
+#ifndef NB200_SOLVE_TMA_IDX_STAGES4
+#define NB200_SOLVE_TMA_IDX_STAGES4 3   // A/B switch (tools/ab_build.py): stages of the sigma-index form with 4 rows
+#endif
+template <int VARIANT, int BM>
 SolveKernel pick_solve_tma_kernel(int maxm, size_t *smem)
 {
-    constexpr size_t nb = SB ? 3 : 5;
-    switch (maxm) {
-    case 1: *smem = 3 * (nb + 1) * kChunkBytes; return dual_solve_tma_kernel<VARIANT, 1, 3, 3, SB>;
-    case 2: *smem = 2 * (nb + 2) * kChunkBytes; return dual_solve_tma_kernel<VARIANT, 2, 2, 3, SB>;
-    case 4:
-        if (SB) { *smem = 3 * (nb + 4) * kChunkBytes; return dual_solve_tma_kernel<VARIANT, 4, 3, 2, SB>; }
-        *smem = 2 * (nb + 4) * kChunkBytes; return dual_solve_tma_kernel<VARIANT, 4, 2, 3, SB>;
-    default: *smem = 0; return nullptr;
+    constexpr size_t stage = (BM == kBoundArrays ? 5 : BM == kScalarBounds ? 3 : 2) * (size_t) kChunkBytes + (BM == kSigmaIndex ? kIdxChunkBytes : 0);
+    if constexpr (BM == kSigmaIndex) {      // 4 rows only (DeviceBackend::sigma_index_runs)
+        *smem = NB200_SOLVE_TMA_IDX_STAGES4 * (stage + 4 * kChunkBytes);
+        return maxm == 4 ? dual_solve_tma_kernel<VARIANT, 4, NB200_SOLVE_TMA_IDX_STAGES4, 2, BM> : nullptr;
+    } else {
+        switch (maxm) {
+        case 1: *smem = 3 * (stage + 1 * kChunkBytes); return dual_solve_tma_kernel<VARIANT, 1, 3, 3, BM>;
+        case 2: *smem = 2 * (stage + 2 * kChunkBytes); return dual_solve_tma_kernel<VARIANT, 2, 2, 3, BM>;
+        case 4:
+            if constexpr (BM == kScalarBounds) { *smem = 3 * (stage + 4 * kChunkBytes); return dual_solve_tma_kernel<VARIANT, 4, 3, 2, BM>; }
+            else { *smem = 2 * (stage + 4 * kChunkBytes); return dual_solve_tma_kernel<VARIANT, 4, 2, 3, BM>; }
+        default: *smem = 0; return nullptr;
+        }
     }
+}
+template <int VARIANT>
+SolveKernel pick_solve_tma_kernel1(int bm, int maxm, size_t *smem)
+{
+    return bm == kSigmaIndex ? pick_solve_tma_kernel<VARIANT, kSigmaIndex>(maxm, smem)
+         : bm == kScalarBounds ? pick_solve_tma_kernel<VARIANT, kScalarBounds>(maxm, smem)
+                               : pick_solve_tma_kernel<VARIANT, kBoundArrays>(maxm, smem);
 }
 
 // asynchronous operand pipeline (dual_solve_async_kernel): {stages} x (5 + rows) x 4 KB of dynamic shared memory per CTA.
@@ -1216,11 +1290,12 @@ bool DeviceBackend::dual_solve(double *y, const double *lo, const double *hi, co
     size_t smem = 0;
     int block = 256;
     SolveKernel fn = nullptr;
-    bool sb = false;
+    bool sb = false, si = false;
     if ((solve_tma_ > 0 || tma_auto) && full && !use_pol && (maxm == 1 || maxm == 2 || maxm == 4)) {
         sb = scalar_bounds_;
-        fn = variant_ == kMMA ? (sb ? pick_solve_tma_kernel<0, true>(maxm, &smem) : pick_solve_tma_kernel<0, false>(maxm, &smem))
-                              : (sb ? pick_solve_tma_kernel<1, true>(maxm, &smem) : pick_solve_tma_kernel<1, false>(maxm, &smem));
+        si = sidx_valid_ && maxm == 4;             // see sigma_index_runs()
+        const int bm = si ? kSigmaIndex : sb ? kScalarBounds : kBoundArrays;
+        fn = variant_ == kMMA ? pick_solve_tma_kernel1<0>(bm, maxm, &smem) : pick_solve_tma_kernel1<1>(bm, maxm, &smem);
         block = kTmaBlock;
         NB_CUDA(cudaFuncSetAttribute((const void *) fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
     } else if (solve_async_ >= 2 && !use_pol && maxm <= 8) {
@@ -1301,7 +1376,7 @@ bool DeviceBackend::dual_solve(double *y, const double *lo, const double *hi, co
     if (Comm::instance().active() && gens > 0) Comm::instance().advance_seq((unsigned long long) gens);
     if (*ret == kRetInvalid) return true;            // nothing ran; the caller reports it
     if (*ret == kRetFailure) return fail("the cross-rank exchange inside the dual solve timed out");
-    count_operand_bytes(gens, sb, true);             // the last generation stored x*(y)
+    count_operand_bytes(gens, sb, si, true);         // the last generation stored x*(y)
     out->val = res_host_[0];
     out->gval = res_host_[1];
     out->wval = res_host_[2];
@@ -1377,16 +1452,22 @@ bool DeviceBackend::end_outer(unsigned k, double sigma_min, double *dnorm, doubl
     a.out_host = out_host_; a.flag_host = flag_host_;
     a.seq = seq_ = Comm::instance().active() ? Comm::instance().next_seq() : seq_ + 1;
     a.publish_host = Comm::instance().active() ? 0 : 1;
-    a.nvp = kEndNvp;               // records of this kernel: 3 sums, stride 4 (its own stride: nvp_ belongs to the dual kernels)
+    a.nvp = kEndNvp;               // records of this kernel: 4 sums (its own stride: nvp_ belongs to the dual kernels)
     a.update_sigma = k > 1;
     a.kappa = variant_ == kMMA ? 0.01 : 1e-8;
     a.sigma_min = sigma_min;
+    if (a.update_sigma && sidx_valid_) {
+        // the palette one update further: the same on every rank, as nothing in it depends on the data
+        sidx_valid_ = sigma_min == sidx_sigma_min_ && palette_.step();
+        if (sidx_valid_ && !upload_palette()) return false;
+        if (sidx_valid_) { a.sidx = sidx_; a.next = next_; a.pal = pal_; }
+    }
     end_outer_kernel<<<(int) geo_.nseg_local, kBlock, 0, stream_>>>(a);
     ++stats_->kernel_launches;
     NB_CUDA(cudaGetLastError());
     if (!a.publish_host) {
         if (Comm::instance().all_gather_inplace(out_dev_, (size_t) geo_.local_vshards * kEndNvp, stream_, &err_)) return false;
-        publish_kernel<<<1, 32, 0, stream_>>>(out_dev_, 3, kEndNvp, out_host_, flag_host_, a.seq);
+        publish_kernel<<<1, 32, 0, stream_>>>(out_dev_, 4, kEndNvp, out_host_, flag_host_, a.seq);
         ++stats_->kernel_launches;
         NB_CUDA(cudaGetLastError());
     }
@@ -1394,6 +1475,11 @@ bool DeviceBackend::end_outer(unsigned k, double sigma_min, double *dnorm, doubl
     *dnorm = out_host_[0];
     *xnorm = out_host_[1];
     *all_below_abs = out_host_[2] == 0.0;
+    if (out_host_[3] != 0.0) {             // a palette value differs from the fp64 sigma: stay on the fp64 path
+        stats_->sigma_index_mismatches += (long long) out_host_[3];
+        sidx_valid_ = false;
+    }
+    stats_->sigma_palette = sidx_valid_ ? (long long) palette_.val.size() : 0;
     return true;
 }
 
@@ -1443,6 +1529,7 @@ bool DeviceBackend::upload(const char *which, const double *host)
     double *dst = array(which);
     if (std::string(which) == "xcur") { dst = xcur_; cand_in_x_ = false; }
     if (!dst) return fail(std::string("unknown array ") + which);
+    if (dst == sigma_) sidx_valid_ = false;
     NB_CUDA(cudaMemcpyAsync(dst, host + geo_.j0, geo_.n_local * sizeof(double), cudaMemcpyHostToDevice, stream_));
     NB_CUDA(cudaStreamSynchronize(stream_));
     return true;

@@ -15,6 +15,11 @@
 
 #include "backend_factory.hpp"
 #include "geometry.hpp"
+#include "sigma_palette.hpp"
+
+#ifndef NB200_SIGMA_INDEX_MIN_MB
+#define NB200_SIGMA_INDEX_MIN_MB 50   // fp64 operand set above which the sigma-index form runs: the L2 (DESIGN.md section 3.2)
+#endif
 
 namespace nb200 {
 
@@ -81,7 +86,9 @@ private:
     void fill_dual_args(struct DualArgs &a, const double *y, const DualScalars &sc);
     bool launch_dual(const double *y, const DualScalars &sc, bool store, bool wait);
     unsigned l2_keep_mask() const;
-    void count_operand_bytes(long long evals, bool sb, bool store);     // nlopt_b200_stats::dual_operand_bytes
+    void count_operand_bytes(long long evals, bool sb, bool si, bool store);     // nlopt_b200_stats::dual_operand_bytes
+    bool upload_palette();
+    bool sigma_index_runs() const;
     bool wait_flag();
     bool host_x_for(Slot slot);                      // bring the slot's x to pinned host memory (cached per epoch)
     bool push_grad_rows(Slot slot, int row0, unsigned rows, bool is_objective, const double *host_grad);
@@ -120,6 +127,18 @@ private:
     // the bounds as two scalars instead of reading the lb / ub arrays, which stay filled for the other kernels
     bool scalar_bounds_ = false;
     double lb_u_ = 0.0, ub_u_ = 0.0;
+    // sigma index: sidx_[j] indexes palette_ (sigma_palette.hpp) and sigma_[j] == palette value, bit for bit, while
+    // sidx_valid_.  Valid from sigma_init_from() with scalar bounds and a uniform initial step; lost for the rest of the
+    // run when sigma is uploaded, the palette would pass its cap, or end_outer_kernel finds a mismatch.  sigma_ stays
+    // the source of truth for every kernel that does not read the index.
+    bool sidx_valid_ = false;
+    unsigned short *sidx_ = nullptr, *next_ = nullptr;      // device: [ld] indices (padding lanes 0), [cap][3] transitions
+    double *pal_ = nullptr;                                 // device: [cap] values
+    double *pal_pinned_ = nullptr;                          // pinned staging of pal_ / next_
+    unsigned short *next_pinned_ = nullptr;
+    SigmaPalette palette_;
+    size_t pal_uploaded_ = 0, rows_uploaded_ = 0;           // palette entries / transition rows already on the device
+    double sidx_sigma_min_ = 0.0;
     int kernel_cfg_ = -1;        // -1: measured default for (variant, m)          // index into the launch-geometry table of device_backend.cu
 
     // device state

@@ -4,7 +4,10 @@ box [-2, 2]^n) for n x m x algorithm, with the box given as two scalars (the ker
 arrays (5 + m).  One point = `--steps` inner iterations after a `--warmup` run, both forms alternated `--reps` times on
 fresh objects; reported per form: microseconds of kernel time per dual evaluation (best rep), the HBM rate of the
 operand bytes the kernels were asked for (nlopt_b200_stats.dual_operand_bytes over seconds_dual_kernel) and f after the
-steps (the forms must agree bit for bit).  Writes build/solve_tma_sweep.json.
+steps (the forms must agree bit for bit), and whether the TMA form read the sigma index (`tma_index`).  To set the
+sigma-index form against the fp64-sigma TMA form, run the sweep again in the same session under
+NLOPT_B200_LIBDIR=build/ab/NAME, a build from tools/ab_build.py with -DNB200_SIGMA_INDEX_MIN_MB=1048576 (the register
+column then shows the drift between the two runs).  Writes build/solve_tma_sweep.json (--out to change).
     python tools/solve_tma_sweep.py [--n 1.25e6,2.5e6,...] [--m 1,4] [--alg mma,ccsaq] [--bounds scalar,array]"""
 import argparse
 import json
@@ -25,6 +28,7 @@ def main():
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--reps", type=int, default=2)
+    ap.add_argument("--out", default=os.path.join(ROOT, "build", "solve_tma_sweep.json"))
     a = ap.parse_args()
     import torch
     import nlopt_b200 as nl
@@ -39,7 +43,8 @@ def main():
         p = Problem()
         p.rosenbrock_device(o, m)
         o.set_param("b200_time_kernels", 1)
-        o.set_param("b200_solve_tma", tma)
+        if not (tma and m == 4 and bounds == "scalar"):   # there the default rule takes the TMA form, with the sigma index
+            o.set_param("b200_solve_tma", tma)            # above NB200_SIGMA_INDEX_MIN_MB; the knob would force fp64 sigma
         xdev = x0dev.clone()
         o.set_maxeval(a.warmup + 1)
         o.optimize_device(xdev.data_ptr())
@@ -49,7 +54,7 @@ def main():
         s = o.get_stats()      # of the last call
         kern = s["seconds_dual_kernel"]
         return dict(us_per_eval=1e6 * kern / max(1, s["dual_evals"]), gbs=s["dual_operand_bytes"] / kern * 1e-9 if kern > 0 else None,
-                    dual_evals=s["dual_evals"], f_hex=float(o.last_optimum_value()).hex())
+                    dual_evals=s["dual_evals"], f_hex=float(o.last_optimum_value()).hex(), sigma_palette=s["sigma_palette"])
 
     rows = []
     for alg in a.alg.split(","):
@@ -68,11 +73,12 @@ def main():
                                tma_speedup=best[0]["us_per_eval"] / best[1]["us_per_eval"],
                                same_f=len({r["f_hex"] for t in res for r in res[t]}) == 1,
                                same_evals=len({r["dual_evals"] for t in res for r in res[t]}) == 1,
+                               tma_index=best[1]["sigma_palette"] > 0,
                                all_us={t: [round(r["us_per_eval"], 2) for r in res[t]] for t in res})
                     rows.append(row)
                     print(json.dumps(row), flush=True)
                 del x0dev
-    out = os.path.join(ROOT, "build", "solve_tma_sweep.json")
+    out = a.out
     os.makedirs(os.path.dirname(out), exist_ok=True)
     json.dump(dict(gpu=torch.cuda.get_device_name(0), rows=rows), open(out, "w"), indent=1)
     print("wrote", out)
