@@ -15,6 +15,14 @@
  * CUDA kernels on sm_90a; there is no CPU fallback (no device =>
  * NLOPT_FAILURE + message).
  *
+ * The AUGLAG family takes device callbacks (objective, inequality and
+ * equality constraints, either form) and nlopt_b200_optimize_device as
+ * well; host and device callbacks may be mixed.  Such a run keeps x and its
+ * best point in HBM and evaluates the outer loop's values on the device
+ * (one GPU only; sharded host callbacks and maximisation with a device
+ * objective are refused).  After any AUGLAG run nlopt_b200_get_stats
+ * reports the last sub-optimisation.
+ *
  * The `nlopt_b200_*` symbols are additive extensions (device-resident
  * callbacks, kernel-level access to the dual evaluation, multi-GPU sharding,
  * statistics).  No torch / CUDA types appear in any signature: device
@@ -214,6 +222,9 @@ typedef double (*nlopt_b200_dfunc)(unsigned n_local, unsigned long long j0, cons
 nlopt_result nlopt_b200_set_min_objective_device(nlopt_opt opt, nlopt_b200_dfunc f, void *f_data);
 nlopt_result nlopt_b200_add_inequality_constraint_device(nlopt_opt opt, nlopt_b200_dfunc fc,
                                                          void *fc_data, double tol);
+/* h(x) = 0 within tol: accepted by the algorithms that take nlopt_add_equality_constraint (the AUGLAG family here);
+ * NLOPT_INVALID_ARGS on LD_MMA / LD_CCSAQ, for a NULL callback or a negative tol */
+nlopt_result nlopt_b200_add_equality_constraint_device(nlopt_opt opt, nlopt_b200_dfunc h, void *h_data, double tol);
 
 /* Device callbacks, second form: asynchronous and independent of the number of ranks.
  * The library cuts the n variables into groups and 8 "virtual shards" by a rule that depends on n only (the rule of the
@@ -241,6 +252,10 @@ nlopt_result nlopt_b200_set_min_objective_device2(nlopt_opt opt, nlopt_b200_dfun
                                                   void *f_data, int halo);
 nlopt_result nlopt_b200_add_inequality_constraint_device2(nlopt_opt opt, nlopt_b200_dfunc2 fc, nlopt_b200_dfinish finish,
                                                           void *fc_data, double tol, int halo);
+/* the equality twin: same argument checks (NULL callback or finish, halo outside {0, 1}, negative tol) and the algorithm
+ * check of nlopt_add_equality_constraint */
+nlopt_result nlopt_b200_add_equality_constraint_device2(nlopt_opt opt, nlopt_b200_dfunc2 h, nlopt_b200_dfinish finish,
+                                                        void *h_data, double tol, int halo);
 /* Sharded HOST callbacks (one process per GPU): the callback sees only this rank's variables -- x_shard and grad_shard
  * hold the n_local entries starting at global index j0 -- and returns its ADDITIVE contribution to the function value
  * (a constant term is added by one rank only, e.g. the one with j0 == 0); the library sums the contributions over the
@@ -254,7 +269,8 @@ nlopt_result nlopt_b200_add_inequality_constraint_sharded(nlopt_opt opt, nlopt_b
 /* like nlopt_optimize, but x_dev is a device array of this rank's shard (in/out) */
 nlopt_result nlopt_b200_optimize_device(nlopt_opt opt, double *x_dev, double *opt_f);
 
-/* Run statistics of the last nlopt_optimize on this object. */
+/* Run statistics of the last nlopt_optimize on this object; after an NLOPT_AUGLAG* run, those of its last
+ * sub-optimisation. */
 typedef struct {
     long long dual_evals;        /* level-1 dual evaluations (kernel launches of the dual kernel) */
     long long dual_solves;       /* = inner CCSA iterations                                      */

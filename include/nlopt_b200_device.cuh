@@ -24,6 +24,7 @@
 //
 // Usage:   nlopt_b200::set_min_objective(opt, &functor);     // functor must outlive opt
 //          nlopt_b200::add_inequality_constraint(opt, &cfunctor, tol);
+//          nlopt_b200::add_equality_constraint(opt, &hfunctor, tol);      // NLOPT_AUGLAG* only
 //
 // The reduction is deterministic AND independent of the number of ranks: the variables are cut into the library's
 // groups and 8 virtual shards (a function of n alone, nlopt_b200_shard_geometry); one CTA reduces one group with a
@@ -223,6 +224,14 @@ nlopt_result add_inequality_constraint(nlopt_opt opt, const F *f, double tol)
                                                         detail::halo_of<F>::value);
 }
 
+// h(x) = 0 within tol (the AUGLAG family): the same kernels, so the same summation order as the inequality form
+template <class F>
+nlopt_result add_equality_constraint(nlopt_opt opt, const F *f, double tol)
+{
+    return nlopt_b200_add_equality_constraint_device2(opt, &detail::trampoline2<F>, &detail::finish2<F>, const_cast<F *>(f), tol,
+                                                      detail::halo_of<F>::value);
+}
+
 // the first form of the interface (one synchronous evaluation per call, nlopt_b200_dfunc), kept for callers that
 // want a value right away: rank-local sums, summed over ranks by the library
 template <class F>
@@ -237,6 +246,13 @@ nlopt_result add_inequality_constraint_sync(nlopt_opt opt, const F *f, double to
 {
     auto *b = new detail::Bound<F>{f, nlopt_get_dimension(opt)};
     return nlopt_b200_add_inequality_constraint_device(opt, &detail::trampoline<F>, b, tol);
+}
+
+template <class F>
+nlopt_result add_equality_constraint_sync(nlopt_opt opt, const F *f, double tol)
+{
+    auto *b = new detail::Bound<F>{f, nlopt_get_dimension(opt)};
+    return nlopt_b200_add_equality_constraint_device(opt, &detail::trampoline<F>, b, tol);
 }
 
 }  // namespace nlopt_b200

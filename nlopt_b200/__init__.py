@@ -185,6 +185,10 @@ class opt:
         self._check(self._lib.nlopt_b200_add_inequality_constraint_device(
             self._h, fn_ptr, data_ptr, float(tol)))
 
+    def add_equality_constraint_device(self, fn_ptr, data_ptr=None, tol=0.0):
+        self._check(self._lib.nlopt_b200_add_equality_constraint_device(
+            self._h, fn_ptr, data_ptr, float(tol)))
+
     def optimize_device(self, x_dev_ptr):
         f = C.c_double(0.0)
         self._exc = None

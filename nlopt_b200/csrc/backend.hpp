@@ -92,8 +92,22 @@ public:
     // (mma.c:431-442) and the rotation xprevprev <- xprev, xprev <- xcur (mma.c:264-265).
     virtual bool end_outer(unsigned k, double sigma_min, double *dnorm, double *xnorm, bool *all_below_abs) = 0;
 
-    // copy the accepted point to host memory (or a device pointer in device mode)
+    // copy the accepted point to host memory (or a device pointer in device mode); values-only backends: the best point
     virtual bool fetch_x(double *x_out) = 0;
+
+    // Values-only backends (BackendConfig::values_only: the outer loop of NLOPT_AUGLAG*) hold a point x and a best
+    // point, and evaluate the functions at x with eval_objective / eval_constraint (kBase, no gradient) + finish_evals.
+    // point_device(): the device array of x; a caller that overwrites it calls point_moved() before the next evaluation.
+    virtual double *point_device() { return nullptr; }
+    virtual void point_moved() {}
+    // nlopt_stop_x between x and the best point (stop.c:98-108, the sums of end_outer), then best <- x: one pass
+    virtual bool stop_x_keep(double *dnorm, double *xnorm, bool *all_below_abs)
+    {
+        (void) dnorm; (void) xnorm; (void) all_below_abs;
+        return false;
+    }
+    // number of ranks the state is sharded over
+    virtual int ranks() const { return 1; }
 
     // Collective OR of a rank-local decision (time limits): with one rank, the identity.  Every rank of a sharded
     // run calls it at the same points of the loop.

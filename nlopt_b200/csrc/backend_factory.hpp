@@ -52,6 +52,7 @@ struct BackendConfig {
     const double *x_weights = nullptr;       // host or null
     const double *xtol_abs = nullptr;        // host or null
     nlopt_b200_stats *stats = nullptr;       // h2d/d2h bytes, launches, kernel time
+    bool values_only = false;                // x, the best point and the callback workspace only (Backend::point_device)
 };
 
 Backend *make_backend(const BackendConfig &cfg, std::string *err);

@@ -2339,6 +2339,8 @@ __global__ void sigma_init_kernel(double *sigma, const double *lb, const double 
 }
 
 // ---- fused end-of-outer-iteration pass -------------------------------------------------------------
+// Also the stop test + "keep the point" of the NLOPT_AUGLAG* outer loop (DeviceBackend::stop_x_keep): update_sigma = 0
+// and a null xprevprev, so xprev (the best point) <- xcur and nothing else is written.
 struct EndOuterArgs {
     const double *xcur;
     double *xprev, *xprevprev, *sigma;
@@ -2411,7 +2413,7 @@ __global__ void __launch_bounds__(kBlock) end_outer_kernel(const __grid_constant
                         acc[3] = addx(acc[3], 1.0);
                 }
             }
-            a.xprevprev[j] = xp;
+            if (a.xprevprev) a.xprevprev[j] = xp;
             a.xprev[j] = xc;
         }
     }

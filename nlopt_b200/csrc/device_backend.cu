@@ -276,6 +276,14 @@ bool DeviceBackend::alloc_state()
     NB_CUDA(cudaStreamCreateWithFlags(&copy_stream_, cudaStreamNonBlocking));
 
     const size_t ld = geo_.ld;
+    if (cfg_.values_only) {                  // x | best point
+        pool_bytes_ = (2 * ld + 3 * kGuard) * sizeof(double);
+        NB_CUDA(cached_malloc(&pool_, pool_bytes_));
+        NB_CUDA(cudaMemsetAsync(pool_, 0, pool_bytes_, stream_));
+        x_ = pool_ + kGuard;
+        xprev_ = x_ + ld + kGuard;
+        return alloc_workspace();
+    }
     // x and xcur carry kGuard cells on either side: the halo of stencil device callbacks (x[-1], x[ld]); everything
     // stays 64-byte aligned (ld is a multiple of 512 doubles)
     const size_t total = (9 + 2 * (size_t) m_) * ld + 3 * kGuard;
@@ -395,6 +403,20 @@ bool DeviceBackend::setup(const BackendConfig &cfg)
     if (cfg.stats) stats_ = cfg.stats;
     if (!alloc_state()) return false;
     const size_t nl = geo_.n_local, j0 = geo_.j0;
+    if (cfg.values_only) {
+        bool any_host_cb = cfg.objective.f != nullptr;
+        for (const FuncSpec &c : cfg.constraints) any_host_cb = any_host_cb || c.f || c.mf;
+        if (any_host_cb) NB_CUDA(cached_host_alloc(&h_x_, (size_t) geo_.n * sizeof(double)));
+        if (cfg.x0_host) {
+            NB_CUDA(cudaMemcpyAsync(x_, cfg.x0_host + j0, nl * sizeof(double), cudaMemcpyHostToDevice, stream_));
+            stats_->h2d_bytes += nl * sizeof(double);
+        } else if (cfg.x_dev) {
+            NB_CUDA(cudaMemcpyAsync(x_, cfg.x_dev, nl * sizeof(double), cudaMemcpyDeviceToDevice, stream_));
+        } else
+            return fail("no start point");
+        NB_CUDA(cudaMemcpyAsync(xprev_, x_, nl * sizeof(double), cudaMemcpyDeviceToDevice, stream_));
+        return set_norm_arrays(cfg.x_weights, cfg.xtol_abs);
+    }
     if (pen_total_) {
         NB_CUDA(cached_malloc(&pen_rows_, (size_t) pen_total_ * geo_.ld * sizeof(double)));
         NB_CUDA(cudaMemsetAsync(pen_rows_, 0, (size_t) pen_total_ * geo_.ld * sizeof(double), stream_));
@@ -619,12 +641,24 @@ bool DeviceBackend::eval_objective(Slot slot, bool want_grad, double *value)
 // The augmented-Lagrangian objective (PenaltySpec, backend_factory.hpp; auglag.c:25-65).  The constraint gradients
 // go to scratch rows in HBM (uploaded through the same pinned staging pipeline as everything else, or written by
 // device callbacks); one kernel then adds the active ones to grad f.  Only the m' + p' values visit the host.
+// Asynchronous device callbacks (the objective and nlopt_b200_dfunc2 constraints) are enqueued back to back and settled
+// by one finish_evals; the penalty rows take the value slots 1 + m + row of that block.
 bool DeviceBackend::eval_penalty_objective(Slot slot, bool want_grad, double *value)
 {
     const PenaltySpec &ps = *cfg_.penalty;
     double L = 0;
     if (!eval_user_objective(slot, want_grad, &L)) return false;
-    if (!finish_evals(&L, nullptr)) return false;
+    std::vector<double> settled(m_ + (size_t) pen_total_ + 1);   // finish_evals' view: [m] constraints | [pen_total_] rows
+    {
+        unsigned row = 0;
+        for (int pass = 0; pass < 2; ++pass)
+            for (const FuncSpec &fs : (pass == 0 ? ps.eq : ps.ineq)) {
+                if (fs.df2 && !enqueue_df2(fs, slot, want_grad ? pen_rows_ + (size_t) row * geo_.ld : nullptr, 1 + m_ + row))
+                    return false;
+                row += fs.m;
+            }
+    }
+    if (!finish_evals(&L, settled.data())) return false;
     if (ps.nevals_p) ++*ps.nevals_p;
     *value = L;
     if (ps.force_stop && *ps.force_stop) return true;               // auglag.c:39
@@ -636,7 +670,9 @@ bool DeviceBackend::eval_penalty_objective(Slot slot, bool want_grad, double *va
     bool any_partial = false;
     for (int pass = 0; pass < 2; ++pass)
         for (const FuncSpec &fs : (pass == 0 ? ps.eq : ps.ineq)) {
-            if (fs.df) {
+            if (fs.df2) {
+                vals[row] = settled[m_ + row];
+            } else if (fs.df) {
                 const double t0 = wall_seconds();
                 vals[row] = fs.df((unsigned) geo_.n_local, geo_.j0, xs, want_grad ? pen_rows_ + (size_t) row * geo_.ld : nullptr, fs.data, stream_);
                 cb_seconds_ += wall_seconds() - t0;
@@ -827,7 +863,7 @@ bool DeviceBackend::enqueue_df2(const FuncSpec &fs, Slot slot, double *grad_dst,
 {
     Comm &comm = Comm::instance();
     if (!vs2_dev_) {
-        vs2_cap_ = 1 + (size_t) m_;
+        vs2_cap_ = 1 + (size_t) m_ + pen_total_;       // objective | constraints | penalty rows (eval_penalty_objective)
         if (!small_dev((void **) &vs2_dev_, vs2_cap_ * kV * sizeof(double))) return false;
         if (!small_pinned((void **) &vs2_host_, vs2_cap_ * kV * sizeof(double))) return false;
         shard_.n = geo_.n; shard_.n_local = geo_.n_local; shard_.j0 = geo_.j0;
@@ -1445,14 +1481,7 @@ bool DeviceBackend::end_outer(unsigned k, double sigma_min, double *dnorm, doubl
     std::memset(&a, 0, sizeof a);
     a.xcur = xcur_view();
     a.xprev = xprev_; a.xprevprev = xprevprev_; a.sigma = sigma_;
-    a.lb = lb_; a.ub = ub_; a.w = w_dev_; a.xtol_abs = xtol_abs_dev_;
-    a.n_local = geo_.n_local; a.nchunks = geo_.nchunks; a.chunk0 = geo_.chunk0;
-    a.nseg_total = geo_.S; a.seg0 = geo_.seg0; a.segs_per_vshard = geo_.P; a.local_vshards = geo_.local_vshards;
-    a.partials = partials_; a.vsums = vsums_; a.tickets = tickets_; a.out_dev = out_dev_;
-    a.out_host = out_host_; a.flag_host = flag_host_;
-    a.seq = seq_ = Comm::instance().active() ? Comm::instance().next_seq() : seq_ + 1;
-    a.publish_host = Comm::instance().active() ? 0 : 1;
-    a.nvp = kEndNvp;               // records of this kernel: 4 sums (its own stride: nvp_ belongs to the dual kernels)
+    a.lb = lb_; a.ub = ub_;
     a.update_sigma = k > 1;
     a.kappa = variant_ == kMMA ? 0.01 : 1e-8;
     a.sigma_min = sigma_min;
@@ -1462,6 +1491,26 @@ bool DeviceBackend::end_outer(unsigned k, double sigma_min, double *dnorm, doubl
         if (sidx_valid_ && !upload_palette()) return false;
         if (sidx_valid_) { a.sidx = sidx_; a.next = next_; a.pal = pal_; }
     }
+    if (!end_outer_pass(a, dnorm, xnorm, all_below_abs)) return false;
+    if (out_host_[3] != 0.0) {             // a palette value differs from the fp64 sigma: stay on the fp64 path
+        stats_->sigma_index_mismatches += (long long) out_host_[3];
+        sidx_valid_ = false;
+    }
+    stats_->sigma_palette = sidx_valid_ ? (long long) palette_.val.size() : 0;
+    return true;
+}
+
+// end_outer_kernel over this rank's groups with the caller's arrays and sigma fields; the three stop sums come back
+bool DeviceBackend::end_outer_pass(EndOuterArgs &a, double *dnorm, double *xnorm, bool *all_below_abs)
+{
+    a.w = w_dev_; a.xtol_abs = xtol_abs_dev_;
+    a.n_local = geo_.n_local; a.nchunks = geo_.nchunks; a.chunk0 = geo_.chunk0;
+    a.nseg_total = geo_.S; a.seg0 = geo_.seg0; a.segs_per_vshard = geo_.P; a.local_vshards = geo_.local_vshards;
+    a.partials = partials_; a.vsums = vsums_; a.tickets = tickets_; a.out_dev = out_dev_;
+    a.out_host = out_host_; a.flag_host = flag_host_;
+    a.seq = seq_ = Comm::instance().active() ? Comm::instance().next_seq() : seq_ + 1;
+    a.publish_host = Comm::instance().active() ? 0 : 1;
+    a.nvp = kEndNvp;               // records of this kernel: 4 sums (its own stride: nvp_ belongs to the dual kernels)
     end_outer_kernel<<<(int) geo_.nseg_local, kBlock, 0, stream_>>>(a);
     ++stats_->kernel_launches;
     NB_CUDA(cudaGetLastError());
@@ -1475,17 +1524,31 @@ bool DeviceBackend::end_outer(unsigned k, double sigma_min, double *dnorm, doubl
     *dnorm = out_host_[0];
     *xnorm = out_host_[1];
     *all_below_abs = out_host_[2] == 0.0;
-    if (out_host_[3] != 0.0) {             // a palette value differs from the fp64 sigma: stay on the fp64 path
-        stats_->sigma_index_mismatches += (long long) out_host_[3];
-        sidx_valid_ = false;
-    }
-    stats_->sigma_palette = sidx_valid_ ? (long long) palette_.val.size() : 0;
     return true;
 }
+
+// The AUGLAG outer loop's acceptance (auglag.c:270-285): the sums of nlopt_stop_x between x and the best point, then
+// best <- x, in one read of both arrays (the end-of-iteration kernel without its sigma update and rotation)
+bool DeviceBackend::stop_x_keep(double *dnorm, double *xnorm, bool *all_below_abs)
+{
+    EndOuterArgs a;
+    std::memset(&a, 0, sizeof a);
+    a.xcur = x_;
+    a.xprev = xprev_;
+    return end_outer_pass(a, dnorm, xnorm, all_below_abs);
+}
+
+int DeviceBackend::ranks() const { return Comm::instance().active() ? Comm::instance().world : 1; }
 
 bool DeviceBackend::fetch_x(double *x_out)
 {
     drain_events();
+    if (cfg_.values_only) {
+        NB_CUDA(cudaMemcpyAsync(x_out, xprev_, geo_.n_local * sizeof(double), cfg_.x_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, stream_));
+        NB_CUDA(cudaStreamSynchronize(stream_));
+        if (!cfg_.x_dev) stats_->d2h_bytes += geo_.n_local * sizeof(double);
+        return true;
+    }
     if (cfg_.x_dev && x_out == cfg_.x_dev) {
         NB_CUDA(cudaMemcpyAsync(x_out, x_, geo_.n_local * sizeof(double), cudaMemcpyDeviceToDevice, stream_));
         NB_CUDA(cudaStreamSynchronize(stream_));

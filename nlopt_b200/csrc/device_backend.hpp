@@ -27,6 +27,7 @@ namespace nb200 {
 //   x xcur xprev xprevprev lb ub sigma grad_f grad_f_cur | grad_c[m][ld] | grad_c_cur[m][ld]
 // ld = shard length rounded up to 32 doubles, so every array and every row is 256-byte aligned.
 // Padding lanes carry sigma = 0, which both dual formulas skip (mma.c:96-99).
+// A values-only backend (BackendConfig::values_only) allocates x (with its guard cells) and xprev (the best point) only.
 class DeviceBackend : public Backend {
 public:
     DeviceBackend();
@@ -59,6 +60,10 @@ public:
     bool first_outer() override;
     bool end_outer(unsigned k, double sigma_min, double *dnorm, double *xnorm, bool *all_below_abs) override;
     bool fetch_x(double *x_out) override;
+    double *point_device() override { return cfg_.values_only ? x_ : nullptr; }
+    void point_moved() override { ++x_epoch_; }
+    bool stop_x_keep(double *dnorm, double *xnorm, bool *all_below_abs) override;
+    int ranks() const override;
     const std::string &error() const override { return err_; }
     double seconds_in_callbacks() const override { return cb_seconds_; }
 
@@ -85,6 +90,7 @@ private:
     double *xcur_view() { return cand_in_x_ ? x_ : xcur_; }
     void fill_dual_args(struct DualArgs &a, const double *y, const DualScalars &sc);
     bool launch_dual(const double *y, const DualScalars &sc, bool store, bool wait);
+    bool end_outer_pass(struct EndOuterArgs &a, double *dnorm, double *xnorm, bool *all_below_abs);
     unsigned l2_keep_mask() const;
     void count_operand_bytes(long long evals, bool sb, bool si, bool store);     // nlopt_b200_stats::dual_operand_bytes
     bool upload_palette();

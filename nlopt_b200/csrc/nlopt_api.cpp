@@ -8,6 +8,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <new>
 
 #include "backend_factory.hpp"
@@ -171,7 +172,7 @@ double flipped(unsigned n, const double *x, double *grad, void *p)
 
 nlopt_result run_ccsa(nlopt_opt opt, double *x_host, double *x_dev, double *minf);
 nlopt_result run_ccsa_precond(nlopt_opt opt, double *x, double *minf, const nb200::CcsaParams &prm);
-nlopt_result run_auglag(nlopt_opt opt, double *x_host, double *minf);
+nlopt_result run_auglag(nlopt_opt opt, double *x_host, double *x_dev, double *minf);
 
 }  // namespace
 
@@ -538,6 +539,20 @@ nlopt_result nlopt_add_precond_equality_constraint(nlopt_opt opt, nlopt_func h, 
 { return add_any(opt, true, false, 1, h, nullptr, nullptr, pre, d, &tol); }
 nlopt_result nlopt_add_equality_constraint(nlopt_opt opt, nlopt_func h, void *d, double tol)
 { return add_any(opt, true, false, 1, h, nullptr, nullptr, nullptr, d, &tol); }
+nlopt_result nlopt_b200_add_equality_constraint_device(nlopt_opt opt, nlopt_b200_dfunc h, void *d, double tol)
+{ return add_any(opt, true, false, 1, nullptr, nullptr, h, nullptr, d, &tol); }
+nlopt_result nlopt_b200_add_equality_constraint_device2(nlopt_opt opt, nlopt_b200_dfunc2 h, nlopt_b200_dfinish fin, void *d,
+                                                        double tol, int halo)
+{
+    if (!h || !fin || halo < 0 || halo > 1) return NLOPT_INVALID_ARGS;
+    nlopt_result r = add_any(opt, true, false, 1, nullptr, nullptr, df2_marker, nullptr, d, &tol);
+    if (r < 0) return r;
+    nb200::ConstraintRec &c = opt->h.back();
+    c.df2 = h;
+    c.dfin = fin;
+    c.halo = halo;
+    return r;
+}
 
 /* ------------------------------------------------------------------ stopping criteria (options.c:661-816) */
 
@@ -765,13 +780,9 @@ static nlopt_result optimize_common(nlopt_opt opt, double *x_host, double *x_dev
         opt->maximize = 0;
     }
     nlopt_result ret;
-    if (is_auglag(opt->algorithm)) {
-        if (!x_host || opt->df) {
-            set_err(opt, "NLOPT_AUGLAG* takes host x and host callbacks in this library");
-            ret = NLOPT_INVALID_ARGS;
-        } else
-            ret = run_auglag(opt, x_host, opt_f);
-    } else
+    if (is_auglag(opt->algorithm))
+        ret = run_auglag(opt, x_host, x_dev, opt_f);
+    else
         ret = run_ccsa(opt, x_host, x_dev, opt_f);
     if (maximize) {
         opt->maximize = maximize;
@@ -1307,31 +1318,45 @@ void eval_values(const nb200::ConstraintRec &c, unsigned n, const double *x, dou
     else c.mf(c.m, out, n, x, nullptr, c.f_data);
 }
 
-nlopt_result optimize_limited(nlopt_opt sub, double *x, double *minf, int maxeval, double maxtime)   // optimize.c:1087-1113
+// x_dev: the sub-problem starts from (and returns into) this device array instead of host x
+nlopt_result optimize_limited(nlopt_opt sub, double *x, double *x_dev, double *minf, int maxeval, double maxtime)   // optimize.c:1087-1113
 {
     const int save_maxeval = sub->maxeval;
     const double save_maxtime = sub->maxtime;
     if (save_maxeval <= 0 || (maxeval > 0 && maxeval < save_maxeval)) sub->maxeval = maxeval;
     if (save_maxtime <= 0 || (maxtime > 0 && maxtime < save_maxtime)) sub->maxtime = maxtime;
-    const nlopt_result ret = nlopt_optimize(sub, x, minf);
+    const nlopt_result ret = x_dev ? nlopt_b200_optimize_device(sub, x_dev, minf) : nlopt_optimize(sub, x, minf);
     sub->maxeval = save_maxeval;
     sub->maxtime = save_maxtime;
     return ret;
 }
 
-nlopt_result run_auglag(nlopt_opt opt, double *x, double *minf)
+// A run whose x is on the device (x_dev, nlopt_b200_optimize_device) or that has a device callback takes the device
+// outer loop: xcur and the best x live in HBM in a values-only backend, each sub-problem is nlopt_b200_optimize_device on
+// xcur, and f, h and c are evaluated at xcur as values only, settled with one host synchronisation (host callbacks of a
+// mixed run see x copied down once per evaluation).  Host x is uploaded once and downloaded once.  Both loops share the
+// scalar logic below.
+nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
 {
     const unsigned n = opt->n;
     const nlopt_algorithm alg = opt->algorithm;
-    if (opt->maximize) { set_err(opt, "NULL args to nlopt_optimize_"); return NLOPT_INVALID_ARGS; }
+    if (opt->maximize || (!x && !x_dev)) { set_err(opt, "NULL args to nlopt_optimize_"); return NLOPT_INVALID_ARGS; }
+    bool dev = x_dev != nullptr || opt->df != nullptr, sharded = opt->sf != nullptr;
     for (const auto *list : {&opt->fc, &opt->h})
-        for (const auto &c : *list)
-            if (c.df) { set_err(opt, "NLOPT_AUGLAG* takes host callbacks in this library"); return NLOPT_INVALID_ARGS; }
-    for (unsigned i = 0; i < n; ++i)                 /* optimize.c:547-551 */
-        if (opt->lb[i] > opt->ub[i] || x[i] < opt->lb[i] || x[i] > opt->ub[i]) {
-            set_err(opt, "bounds %d fail %g <= %g <= %g", (int) i, opt->lb[i], x[i], opt->ub[i]);
-            return NLOPT_INVALID_ARGS;
+        for (const auto &c : *list) {
+            dev = dev || c.df;
+            sharded = sharded || c.sf;
         }
+    if (sharded) {
+        set_err(opt, "NLOPT_AUGLAG* does not take sharded host callbacks (nlopt_b200_sfunc) in this library");
+        return NLOPT_INVALID_ARGS;
+    }
+    if (x)
+        for (unsigned i = 0; i < n; ++i)             /* optimize.c:547-551 */
+            if (opt->lb[i] > opt->ub[i] || x[i] < opt->lb[i] || x[i] > opt->ub[i]) {
+                set_err(opt, "bounds %d fail %g <= %g <= %g", (int) i, opt->lb[i], x[i], opt->ub[i]);
+                return NLOPT_INVALID_ARGS;
+            }
     if ((alg == NLOPT_AUGLAG || alg == NLOPT_AUGLAG_EQ) && !opt->local_opt) {
         set_err(opt, "local optimizer must be specified for AUGLAG");
         return NLOPT_INVALID_ARGS;
@@ -1381,7 +1406,7 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *minf)
     std::vector<double> lambda(pp ? pp : 1, 0.0), mu(mm ? mm : 1, 0.0);
     auto to_spec = [](const nb200::ConstraintRec &c) {
         nb200::FuncSpec s;
-        s.m = c.m; s.f = c.f; s.mf = c.mf; s.data = c.f_data;
+        s.m = c.m; s.f = c.f; s.mf = c.mf; s.df = c.df; s.df2 = c.df2; s.dfin = c.dfin; s.halo = c.halo; s.data = c.f_data;
         return s;
     };
     for (const auto &c : opt->h) pen.eq.push_back(to_spec(c));
@@ -1396,7 +1421,10 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *minf)
        objective, the rest as the penalty spec */
     sub->f = opt->f;
     sub->f_data = opt->f_data;
-    sub->df = nullptr;
+    sub->df = opt->df;
+    sub->df2 = opt->df2;
+    sub->dfin = opt->dfin;
+    sub->halo = opt->halo;
     sub->pre = nullptr;
     sub->maximize = 0;
     nlopt_set_lower_bounds(sub, opt->lb.data());
@@ -1415,128 +1443,201 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *minf)
         sub->munge_on_copy = mc;
     }
     for (const auto &c : sub_fc) {
-        nlopt_result r = c.f ? nlopt_add_inequality_constraint(sub, c.f, c.f_data, c.tol[0])
-                             : nlopt_add_inequality_mconstraint(sub, c.m, c.mf, c.f_data, c.tol.data());
+        nlopt_result r = c.df2 ? nlopt_b200_add_inequality_constraint_device2(sub, c.df2, c.dfin, c.f_data, c.tol[0], c.halo)
+                       : c.df  ? nlopt_b200_add_inequality_constraint_device(sub, c.df, c.f_data, c.tol[0])
+                       : c.f   ? nlopt_add_inequality_constraint(sub, c.f, c.f_data, c.tol[0])
+                               : nlopt_add_inequality_mconstraint(sub, c.m, c.mf, c.f_data, c.tol.data());
         if (r < 0) return r;
     }
     sub->penalty = &pen;
 
+    /* the device outer loop's xcur, best x and callback workspace: objective, then h, then the penalty inequalities */
+    std::unique_ptr<nb200::Backend> ev;
+    nlopt_b200_stats ev_stats{};
+    if (dev) {
+        nb200::BackendConfig vc;
+        vc.values_only = true;
+        vc.n = n;
+        vc.objective.f = opt->f; vc.objective.df = opt->df; vc.objective.df2 = opt->df2; vc.objective.dfin = opt->dfin;
+        vc.objective.halo = opt->halo; vc.objective.data = opt->f_data;
+        for (const auto &c : opt->h) vc.constraints.push_back(to_spec(c));
+        for (const auto &c : pen_fc) vc.constraints.push_back(to_spec(c));
+        vc.lb = opt->lb.data();
+        vc.ub = opt->ub.data();
+        vc.x0_host = x;
+        vc.x_dev = x_dev;
+        vc.x_weights = opt->has_x_weights ? opt->x_weights.data() : nullptr;
+        vc.xtol_abs = opt->has_xtol_abs ? opt->xtol_abs.data() : nullptr;
+        vc.stats = &ev_stats;
+        std::string err;
+        ev.reset(nb200::make_backend(vc, &err));
+        if (!ev) { set_err(opt, "%s", err.c_str()); return NLOPT_FAILURE; }
+        if (ev->ranks() > 1) {   /* DESIGN.md section 8 */
+            set_err(opt, "NLOPT_AUGLAG* with device callbacks or device x runs on one GPU in this library");
+            return NLOPT_INVALID_ARGS;
+        }
+    }
+
     const double t_start = nb200::wall_seconds();
     auto forced = [&] { return opt->force_stop != 0; };
-    std::vector<double> xcur(x, x + n), vals;
-    unsigned maxdim = 1;
-    for (const auto &c : pen_fc) maxdim = c.m > maxdim ? c.m : maxdim;
-    for (const auto &c : opt->h) maxdim = c.m > maxdim ? c.m : maxdim;
-    vals.resize(maxdim);
+    std::vector<double> xcur, hv(pp ? pp : 1), cv(mm ? mm : 1), dv(pp + mm + 1);
+    if (!dev) xcur.assign(x, x + n);
+
+    // f, h and c at xcur (auglag.c:159-170, :212-240), values only; NLOPT_FORCED_STOP as soon as a callback asks for it
+    auto eval_point = [&](double *f) -> nlopt_result {
+        ++opt->numevals;
+        if (!dev) {
+            *f = opt->f(n, xcur.data(), nullptr, opt->f_data);
+            if (forced()) return NLOPT_FORCED_STOP;
+            unsigned i = 0;
+            for (const auto &c : opt->h) {
+                eval_values(c, n, xcur.data(), hv.data() + i);
+                i += c.m;
+                if (forced()) return NLOPT_FORCED_STOP;
+            }
+            i = 0;
+            for (const auto &c : pen_fc) {
+                eval_values(c, n, xcur.data(), cv.data() + i);
+                i += c.m;
+                if (forced()) return NLOPT_FORCED_STOP;
+            }
+            return NLOPT_SUCCESS;
+        }
+        bool ok = ev->eval_objective(nb200::kBase, false, f);
+        if (ok && forced()) return NLOPT_FORCED_STOP;
+        for (unsigned ic = 0, row = 0; ok && ic < ev->num_constraint_objects(); row += ev->constraint_dim(ic++)) {
+            ok = ev->eval_constraint(nb200::kBase, ic, row, false, dv.data() + row);
+            if (ok && forced()) return NLOPT_FORCED_STOP;
+        }
+        if (!ok || !ev->finish_evals(f, dv.data())) {
+            set_err(opt, "outer evaluation: %s", ev->error().c_str());
+            return NLOPT_FAILURE;
+        }
+        std::copy(dv.begin(), dv.begin() + pp, hv.begin());
+        std::copy(dv.begin() + pp, dv.begin() + pp + mm, cv.begin());
+        return NLOPT_SUCCESS;
+    };
+    // nlopt_stop_x(xcur, x) (stop.c:98-108), then x <- xcur
+    auto keep_xcur = [&](bool *stop_x) -> bool {
+        if (!dev) {
+            *stop_x = stop_x_host(opt, xcur.data(), x);
+            std::memcpy(x, xcur.data(), sizeof(double) * n);
+            return true;
+        }
+        double dn, xn;
+        bool below;
+        if (!ev->stop_x_keep(&dn, &xn, &below)) {
+            set_err(opt, "outer stop test: %s", ev->error().c_str());
+            return false;
+        }
+        *stop_x = dn < opt->xtol_rel * xn || (opt->has_xtol_abs && below);
+        return true;
+    };
 
     /* magic parameters from Birgin & Martinez (auglag.c:85-87) */
     const double tau = 0.5, gam = 10, lam_min = -1e20, lam_max = 1e20, mu_max = 1e20;
     double ICM = HUGE_VAL, minf_penalty = HUGE_VAL, penalty = 0, fcur = 0;
     int feasible = 0, minf_feasible = 0;
-    nlopt_result ret = NLOPT_SUCCESS;
     *minf = HUGE_VAL;
 
-    if (pp > 0 || mm > 0) {                          /* starting rho, auglag.c:155-190 */
-        double con2 = 0;
-        ++opt->numevals;
-        fcur = opt->f(n, xcur.data(), nullptr, opt->f_data);
-        if (forced()) return NLOPT_FORCED_STOP;
-        penalty = 0;
-        feasible = 1;
-        for (const auto &c : opt->h) {
-            eval_values(c, n, xcur.data(), vals.data());
-            if (forced()) return NLOPT_FORCED_STOP;
-            for (unsigned k = 0; k < c.m; ++k) {
-                const double hi = vals[k];
-                penalty += std::fabs(hi);
-                feasible = feasible && std::fabs(hi) <= c.tol[k];
-                con2 += hi * hi;
-            }
-        }
-        for (const auto &c : pen_fc) {
-            eval_values(c, n, xcur.data(), vals.data());
-            if (forced()) return NLOPT_FORCED_STOP;
-            for (unsigned k = 0; k < c.m; ++k) {
-                const double fci = vals[k];
-                penalty += fci > 0 ? fci : 0;
-                feasible = feasible && fci <= c.tol[k];
-                if (fci > 0) con2 += fci * fci;
-            }
-        }
-        *minf = fcur;
-        minf_penalty = penalty;
-        minf_feasible = feasible;
-        const double r0 = 2 * std::fabs(*minf) / con2;
-        pen.rho = con2 > 0 ? std::max(1e-6, std::min(10.0, r0)) : 10;
-    } else
-        pen.rho = 1;
     const int verbose = (int) nlopt_get_param(opt, "verbosity", 0);
     int iters = 0;
-
-    do {                                             /* auglag.c:204-296 */
-        const double prev_ICM = ICM;
-        ret = optimize_limited(sub, xcur.data(), &fcur, opt->maxeval - opt->numevals,
-                               opt->maxtime - (nb200::wall_seconds() - t_start));
-        if (ret < 0) {
-            if (sub->has_errmsg) set_err(opt, "%s", sub->errmsg.c_str());
-            break;
-        }
-        ++opt->numevals;
-        fcur = opt->f(n, xcur.data(), nullptr, opt->f_data);
-        if (forced()) return NLOPT_FORCED_STOP;
-        ICM = 0;
-        penalty = 0;
-        feasible = 1;
-        unsigned ii = 0;
-        for (const auto &c : opt->h) {
-            eval_values(c, n, xcur.data(), vals.data());
-            if (forced()) return NLOPT_FORCED_STOP;
-            for (unsigned k = 0; k < c.m; ++k) {
-                const double hi = vals[k];
-                const double newlam = lambda[ii] + pen.rho * hi;
-                penalty += std::fabs(hi);
-                feasible = feasible && std::fabs(hi) <= c.tol[k];
-                ICM = std::max(ICM, std::fabs(hi));
-                lambda[ii++] = std::min(std::max(lam_min, newlam), lam_max);
-            }
-        }
-        ii = 0;
-        for (const auto &c : pen_fc) {
-            eval_values(c, n, xcur.data(), vals.data());
-            if (forced()) return NLOPT_FORCED_STOP;
-            for (unsigned k = 0; k < c.m; ++k) {
-                const double fci = vals[k];
-                const double newmu = mu[ii] + pen.rho * fci;
-                penalty += fci > 0 ? fci : 0;
-                feasible = feasible && fci <= c.tol[k];
-                ICM = std::max(ICM, std::fabs(std::max(fci, -mu[ii] / pen.rho)));
-                mu[ii++] = std::min(std::max(0.0, newmu), mu_max);
-            }
-        }
-        if (ICM > tau * prev_ICM) pen.rho *= gam;
-        ++iters;
-        if (verbose)
-            std::printf("auglag %d: ICM=%g (%sfeasible), rho=%g, fcur=%g\n", iters, ICM, feasible ? "" : "not ", pen.rho, fcur);
-
-        if ((feasible && (!minf_feasible || penalty < minf_penalty || fcur < *minf)) || (!minf_feasible && penalty < minf_penalty)) {
-            ret = NLOPT_SUCCESS;
-            if (feasible) {
-                if (fcur < opt->stopval) ret = NLOPT_STOPVAL_REACHED;
-                else if (rel_stop_host(*minf, fcur, opt->ftol_rel, opt->ftol_abs)) ret = NLOPT_FTOL_REACHED;
-                else if (stop_x_host(opt, xcur.data(), x)) ret = NLOPT_XTOL_REACHED;
-            }
+    auto outer = [&]() -> nlopt_result {
+        nlopt_result ret = NLOPT_SUCCESS;
+        if (pp > 0 || mm > 0) {                      /* starting rho, auglag.c:155-190 */
+            double con2 = 0;
+            if ((ret = eval_point(&fcur)) != NLOPT_SUCCESS) return ret;
+            penalty = 0;
+            feasible = 1;
+            unsigned ii = 0;
+            for (const auto &c : opt->h)
+                for (unsigned k = 0; k < c.m; ++k) {
+                    const double hi = hv[ii++];
+                    penalty += std::fabs(hi);
+                    feasible = feasible && std::fabs(hi) <= c.tol[k];
+                    con2 += hi * hi;
+                }
+            ii = 0;
+            for (const auto &c : pen_fc)
+                for (unsigned k = 0; k < c.m; ++k) {
+                    const double fci = cv[ii++];
+                    penalty += fci > 0 ? fci : 0;
+                    feasible = feasible && fci <= c.tol[k];
+                    if (fci > 0) con2 += fci * fci;
+                }
             *minf = fcur;
             minf_penalty = penalty;
             minf_feasible = feasible;
-            std::memcpy(x, xcur.data(), sizeof(double) * n);
-            if (ret != NLOPT_SUCCESS) break;
-        }
-        if (forced()) { ret = NLOPT_FORCED_STOP; break; }
-        if (opt->maxeval > 0 && opt->numevals >= opt->maxeval) { ret = NLOPT_MAXEVAL_REACHED; break; }
-        if (opt->maxtime > 0 && nb200::wall_seconds() - t_start >= opt->maxtime) { ret = NLOPT_MAXTIME_REACHED; break; }
-        if (ICM == 0) { ret = NLOPT_FTOL_REACHED; break; }
-    } while (true);
-    opt->stats = sub->stats;
+            const double r0 = 2 * std::fabs(*minf) / con2;
+            pen.rho = con2 > 0 ? std::max(1e-6, std::min(10.0, r0)) : 10;
+        } else
+            pen.rho = 1;
+
+        do {                                         /* auglag.c:204-296 */
+            const double prev_ICM = ICM;
+            ret = optimize_limited(sub, xcur.data(), dev ? ev->point_device() : nullptr, &fcur, opt->maxeval - opt->numevals,
+                                   opt->maxtime - (nb200::wall_seconds() - t_start));
+            if (ret < 0) {
+                if (sub->has_errmsg) set_err(opt, "%s", sub->errmsg.c_str());
+                break;
+            }
+            if (dev) ev->point_moved();
+            if ((ret = eval_point(&fcur)) != NLOPT_SUCCESS) return ret;
+            ICM = 0;
+            penalty = 0;
+            feasible = 1;
+            unsigned ii = 0;
+            for (const auto &c : opt->h)
+                for (unsigned k = 0; k < c.m; ++k) {
+                    const double hi = hv[ii];
+                    const double newlam = lambda[ii] + pen.rho * hi;
+                    penalty += std::fabs(hi);
+                    feasible = feasible && std::fabs(hi) <= c.tol[k];
+                    ICM = std::max(ICM, std::fabs(hi));
+                    lambda[ii++] = std::min(std::max(lam_min, newlam), lam_max);
+                }
+            ii = 0;
+            for (const auto &c : pen_fc)
+                for (unsigned k = 0; k < c.m; ++k) {
+                    const double fci = cv[ii];
+                    const double newmu = mu[ii] + pen.rho * fci;
+                    penalty += fci > 0 ? fci : 0;
+                    feasible = feasible && fci <= c.tol[k];
+                    ICM = std::max(ICM, std::fabs(std::max(fci, -mu[ii] / pen.rho)));
+                    mu[ii++] = std::min(std::max(0.0, newmu), mu_max);
+                }
+            if (ICM > tau * prev_ICM) pen.rho *= gam;
+            ++iters;
+            if (verbose)
+                std::printf("auglag %d: ICM=%g (%sfeasible), rho=%g, fcur=%g\n", iters, ICM, feasible ? "" : "not ", pen.rho, fcur);
+
+            if ((feasible && (!minf_feasible || penalty < minf_penalty || fcur < *minf)) || (!minf_feasible && penalty < minf_penalty)) {
+                bool stop_x = false;
+                if (!keep_xcur(&stop_x)) return NLOPT_FAILURE;          /* nlopt_stop_x(xcur, x), x <- xcur */
+                ret = NLOPT_SUCCESS;
+                if (feasible) {
+                    if (fcur < opt->stopval) ret = NLOPT_STOPVAL_REACHED;
+                    else if (rel_stop_host(*minf, fcur, opt->ftol_rel, opt->ftol_abs)) ret = NLOPT_FTOL_REACHED;
+                    else if (stop_x) ret = NLOPT_XTOL_REACHED;
+                }
+                *minf = fcur;
+                minf_penalty = penalty;
+                minf_feasible = feasible;
+                if (ret != NLOPT_SUCCESS) break;
+            }
+            if (forced()) { ret = NLOPT_FORCED_STOP; break; }
+            if (opt->maxeval > 0 && opt->numevals >= opt->maxeval) { ret = NLOPT_MAXEVAL_REACHED; break; }
+            if (opt->maxtime > 0 && nb200::wall_seconds() - t_start >= opt->maxtime) { ret = NLOPT_MAXTIME_REACHED; break; }
+            if (ICM == 0) { ret = NLOPT_FTOL_REACHED; break; }
+        } while (true);
+        opt->stats = sub->stats;
+        return ret;
+    };
+    nlopt_result ret = outer();
+    if (dev && !ev->fetch_x(x ? x : x_dev) && ret > 0) {          /* the best x, once */
+        set_err(opt, "copying the result back failed: %s", ev->error().c_str());
+        ret = NLOPT_FAILURE;
+    }
     return ret;
 }
 

@@ -107,6 +107,25 @@ struct MeanDev {
     double finish(double s) const { return s * inv_n + offset; }
 };
 
+// nonlinear equality mean(x_j^2) - r: term x_j * x_j, gradient 2 x_j, each one IEEE operation
+struct SphereDev {
+    double inv_n, r;
+    __device__ double operator()(unsigned long long, unsigned long long, long long jl, long long, const double *x,
+                                 double *grad_j) const
+    {
+        const double xj = x[jl];
+        if (grad_j) *grad_j = __dmul_rn(2.0, xj);
+        return __dmul_rn(xj, xj);
+    }
+    double finish(double s) const { return s * inv_n - r; }
+};
+
+template <class F>
+int add_eq(nlopt_opt opt, const F *f, double tol, int sync)
+{
+    return sync ? nlopt_b200::add_equality_constraint_sync(opt, f, tol) : nlopt_b200::add_equality_constraint(opt, f, tol);
+}
+
 }  // namespace
 
 struct nb200p_lin_data {
@@ -129,6 +148,7 @@ struct nb200p_problem_s {
     QuadraticDev quad;
     std::vector<LinearDev *> lin;
     std::vector<MeanDev *> mean;
+    std::vector<SphereDev *> sphere;
     std::vector<double *> dev_rows;
     std::vector<nb200p_lin_data *> lin_host;
     SimpDev simp;
@@ -145,6 +165,7 @@ void nb200p_destroy(nb200p_problem_s *p)
     for (double *d : p->dev_rows) cudaFree(d);
     for (LinearDev *l : p->lin) delete l;
     for (MeanDev *m : p->mean) delete m;
+    for (SphereDev *s : p->sphere) delete s;
     for (nb200p_lin_data *l : p->lin_host) delete l;
     for (void *q : p->misc_host) std::free(q);
     delete p;
@@ -159,18 +180,66 @@ int nb200p_set_rosenbrock_device(nb200p_problem_s *p, nlopt_opt opt)
     return nlopt_b200::set_min_objective(opt, &p->rosen);
 }
 
-int nb200p_add_linear_device(nb200p_problem_s *p, nlopt_opt opt, const double *w_host_full, double b, double tol)
+static LinearDev *make_linear(nb200p_problem_s *p, nlopt_opt opt, const double *w_host_full, double b)
 {
     const unsigned n = nlopt_get_dimension(opt);
     unsigned long long j0 = 0, cnt = n;
     nlopt_b200_shard_range(n, nlopt_b200_comm_rank(), nlopt_b200_comm_world(), &j0, &cnt);
     double *w = nullptr;
-    if (cudaMalloc(&w, (cnt ? cnt : 1) * sizeof(double)) != cudaSuccess) return NLOPT_OUT_OF_MEMORY;
+    if (cudaMalloc(&w, (cnt ? cnt : 1) * sizeof(double)) != cudaSuccess) return nullptr;
     cudaMemcpy(w, w_host_full + j0, cnt * sizeof(double), cudaMemcpyHostToDevice);
     p->dev_rows.push_back(w);
     LinearDev *l = new LinearDev{w, b};
     p->lin.push_back(l);
-    return nlopt_b200::add_inequality_constraint(opt, l, tol);
+    return l;
+}
+
+int nb200p_add_linear_device(nb200p_problem_s *p, nlopt_opt opt, const double *w_host_full, double b, double tol)
+{
+    LinearDev *l = make_linear(p, opt, w_host_full, b);
+    return l ? nlopt_b200::add_inequality_constraint(opt, l, tol) : NLOPT_OUT_OF_MEMORY;
+}
+
+// equality constraints (NLOPT_AUGLAG*); sync != 0 registers the synchronous form (nlopt_b200_dfunc)
+int nb200p_add_linear_device_eq(nb200p_problem_s *p, nlopt_opt opt, const double *w_host_full, double b, double tol, int sync)
+{
+    LinearDev *l = make_linear(p, opt, w_host_full, b);
+    return l ? add_eq(opt, l, tol, sync) : NLOPT_OUT_OF_MEMORY;
+}
+
+int nb200p_add_mean_device_eq(nb200p_problem_s *p, nlopt_opt opt, double offset, double tol, int sync)
+{
+    MeanDev *m = new MeanDev{1.0 / (double) nlopt_get_dimension(opt), offset};
+    p->mean.push_back(m);
+    return add_eq(opt, m, tol, sync);
+}
+
+int nb200p_add_sphere_device_eq(nb200p_problem_s *p, nlopt_opt opt, double r, double tol, int sync)
+{
+    SphereDev *s = new SphereDev{1.0 / (double) nlopt_get_dimension(opt), r};
+    p->sphere.push_back(s);
+    return add_eq(opt, s, tol, sync);
+}
+
+// the synchronous forms of the quadratic / SIMP objectives and the mean inequality
+int nb200p_set_quadratic_device_sync(nb200p_problem_s *p, nlopt_opt opt, unsigned long long seed)
+{
+    p->quad.seed = seed;
+    return nlopt_b200::set_min_objective_sync(opt, &p->quad);
+}
+
+int nb200p_set_simp_device_sync(nb200p_problem_s *p, nlopt_opt opt, unsigned long long seed, double eps)
+{
+    p->simp.seed = seed;
+    p->simp.eps = eps;
+    return nlopt_b200::set_min_objective_sync(opt, &p->simp);
+}
+
+int nb200p_add_mean_device_sync(nb200p_problem_s *p, nlopt_opt opt, double offset, double tol)
+{
+    MeanDev *m = new MeanDev{1.0 / (double) nlopt_get_dimension(opt), offset};
+    p->mean.push_back(m);
+    return nlopt_b200::add_inequality_constraint_sync(opt, m, tol);
 }
 
 int nb200p_set_quadratic_device(nb200p_problem_s *p, nlopt_opt opt, unsigned long long seed)

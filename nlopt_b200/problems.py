@@ -26,6 +26,12 @@ def _load():
     L.nb200p_make_linear_data.restype = C.c_void_p
     L.nb200p_make_linear_data.argtypes = [C.c_void_p, c_double_p, C.c_double]
     L.nb200p_set_simp_device.argtypes = [C.c_void_p, C.c_void_p, C.c_ulonglong, C.c_double]
+    L.nb200p_add_linear_device_eq.argtypes = [C.c_void_p, C.c_void_p, c_double_p, C.c_double, C.c_double, C.c_int]
+    L.nb200p_add_mean_device_eq.argtypes = [C.c_void_p, C.c_void_p, C.c_double, C.c_double, C.c_int]
+    L.nb200p_add_sphere_device_eq.argtypes = [C.c_void_p, C.c_void_p, C.c_double, C.c_double, C.c_int]
+    L.nb200p_set_quadratic_device_sync.argtypes = [C.c_void_p, C.c_void_p, C.c_ulonglong]
+    L.nb200p_set_simp_device_sync.argtypes = [C.c_void_p, C.c_void_p, C.c_ulonglong, C.c_double]
+    L.nb200p_add_mean_device_sync.argtypes = [C.c_void_p, C.c_void_p, C.c_double, C.c_double]
     for nm, args in (("nb200p_make_simp_data", [C.c_void_p, C.c_ulonglong, C.c_double]),
                      ("nb200p_make_mean_data", [C.c_void_p, C.c_double]), ("nb200p_make_quad_data", [C.c_void_p, C.c_ulonglong])):
         getattr(L, nm).restype = C.c_void_p
@@ -77,6 +83,46 @@ class Problem:
     def quadratic_device(self, opt, seed=0x5EED0000, offset=0.1, tol=0.0):
         opt._check(self.L.nb200p_set_quadratic_device(self.h, opt._h, seed))
         opt._check(self.L.nb200p_add_mean_device(self.h, opt._h, offset, tol))
+
+    # ---- device functors one at a time; sync=True registers the synchronous form (nlopt_b200_dfunc) ----
+    def set_quadratic_device(self, opt, seed=0x5EED0000, sync=False):
+        fn = self.L.nb200p_set_quadratic_device_sync if sync else self.L.nb200p_set_quadratic_device
+        opt._check(fn(self.h, opt._h, seed))
+
+    def set_simp_device(self, opt, seed=0x5EED0000, eps=1e-3, sync=False):
+        fn = self.L.nb200p_set_simp_device_sync if sync else self.L.nb200p_set_simp_device
+        opt._check(fn(self.h, opt._h, seed, eps))
+
+    def add_mean_device(self, opt, offset, tol=0.0, sync=False):
+        """inequality  mean(x) + offset <= 0"""
+        fn = self.L.nb200p_add_mean_device_sync if sync else self.L.nb200p_add_mean_device
+        opt._check(fn(self.h, opt._h, offset, tol))
+
+    def add_mean_device_eq(self, opt, offset, tol=0.0, sync=False):
+        """equality  mean(x) + offset = 0  (NLOPT_AUGLAG*)"""
+        opt._check(self.L.nb200p_add_mean_device_eq(self.h, opt._h, offset, tol, int(sync)))
+
+    def add_linear_device_eq(self, opt, w, b, tol=0.0, sync=False):
+        """equality  w.x - b = 0  (NLOPT_AUGLAG*)"""
+        w = np.ascontiguousarray(w, dtype=np.float64)
+        opt._check(self.L.nb200p_add_linear_device_eq(self.h, opt._h, w.ctypes.data_as(c_double_p), b, tol, int(sync)))
+
+    def add_sphere_device_eq(self, opt, r, tol=0.0, sync=False):
+        """equality  mean(x_j^2) - r = 0  (NLOPT_AUGLAG*)"""
+        opt._check(self.L.nb200p_add_sphere_device_eq(self.h, opt._h, r, tol, int(sync)))
+
+    def simp_device_eq(self, opt, seed=0x5EED0000, eps=1e-3, vol=0.4, tol=0.0):
+        """config 4 with the volume constraint as an equality, device functors"""
+        self.set_simp_device(opt, seed, eps)
+        self.add_mean_device_eq(opt, -vol, tol)
+
+    def simp_host_eq(self, opt, seed=0x5EED0000, eps=1e-3, vol=0.4, tol=0.0):
+        """config 4 with the volume constraint as an equality, plain C host callbacks"""
+        lib_ = opt._lib
+        d = self.L.nb200p_make_simp_data(self.h, seed, eps)
+        opt._check(lib_.nlopt_set_min_objective(opt._h, self._fn("nb200p_simp_host"), d))
+        dm = self.L.nb200p_make_mean_data(self.h, -vol)
+        opt._check(lib_.nlopt_add_equality_constraint(opt._h, self._fn("nb200p_mean_host"), dm, tol))
 
     # ---- host callbacks in C (any NLopt-ABI library) ----
     def _fn(self, name):
