@@ -256,6 +256,24 @@ nlopt_result nlopt_b200_add_inequality_constraint_device2(nlopt_opt opt, nlopt_b
  * check of nlopt_add_equality_constraint */
 nlopt_result nlopt_b200_add_equality_constraint_device2(nlopt_opt opt, nlopt_b200_dfunc2 h, nlopt_b200_dfinish finish,
                                                         void *h_data, double tol, int halo);
+/* Vector device constraints (the device twin of nlopt_mfunc): one callback produces m constraint rows in one pass over x.
+ * The callback enqueues the m components: vsums_dev is an [m][8] block (row i at vsums_dev + 8 i, zeroed by the
+ * library); it leaves the sum of component i over each of ITS virtual shards in row i, reduced in an order that depends
+ * on n only.  grad_dev: NULL, or row i of the Jacobian at grad_dev + i * grad_ld (this rank's shard).  After all
+ * callbacks of a point have been enqueued, the library adds each row's 8 shard sums in index order and calls
+ * finish(m, totals, result, data) once on the host: result[i] is constraint i.
+ * Argument checks follow nlopt_add_*_mconstraint and the scalar _device2 twins: m == 0 succeeds and registers nothing;
+ * NULL callback or finish and halo outside {0, 1} are NLOPT_INVALID_ARGS; tol (m entries) NULL means zeros; the
+ * equality form is accepted by the algorithms that take nlopt_add_equality_constraint (the AUGLAG family here). */
+typedef void (*nlopt_b200_dmfunc2)(unsigned m, const nlopt_b200_shard *shard, const double *x_dev, double *grad_dev,
+                                   unsigned long long grad_ld, double *vsums_dev, void *func_data, void *cuda_stream);
+typedef void (*nlopt_b200_dmfinish)(unsigned m, const double *totals, double *result, void *func_data);
+nlopt_result nlopt_b200_add_inequality_mconstraint_device2(nlopt_opt opt, unsigned m, nlopt_b200_dmfunc2 fc,
+                                                           nlopt_b200_dmfinish finish, void *fc_data, const double *tol,
+                                                           int halo);
+nlopt_result nlopt_b200_add_equality_mconstraint_device2(nlopt_opt opt, unsigned m, nlopt_b200_dmfunc2 h,
+                                                         nlopt_b200_dmfinish finish, void *h_data, const double *tol,
+                                                         int halo);
 /* Sharded HOST callbacks (one process per GPU): the callback sees only this rank's variables -- x_shard and grad_shard
  * hold the n_local entries starting at global index j0 -- and returns its ADDITIVE contribution to the function value
  * (a constant term is added by one rank only, e.g. the one with j0 == 0); the library sums the contributions over the

@@ -26,6 +26,23 @@
 //          nlopt_b200::add_inequality_constraint(opt, &cfunctor, tol);
 //          nlopt_b200::add_equality_constraint(opt, &hfunctor, tol);      // NLOPT_AUGLAG* only
 //
+// Vector functors: m constraint rows from one visit of each variable (nlopt_b200_dmfunc2), e.g. local volumes:
+//
+//   struct LocalVolumes {
+//       static constexpr int m = 4;                     // 1 <= m <= 16
+//       static constexpr int halo = 0;                  // optional, as for scalar functors
+//       // terms of variable j for the m components into t[0..m-1]; if grad != nullptr, d c_i / d x_j into
+//       // grad[i * grad_ld] (grad already points at variable jl of row 0)
+//       __device__ void operator()(unsigned long long j, unsigned long long n, long long jl, long long n_local,
+//                                  const double *x, double *t, double *grad, long long grad_ld) const;
+//       void finish(const double *totals, double *c) const;   // host: c[i] from the m global totals
+//   };
+//   nlopt_b200::add_inequality_mconstraint(opt, &f, tol /* F::m doubles or nullptr */);
+//   nlopt_b200::add_equality_mconstraint(opt, &f, tol);            // NLOPT_AUGLAG* only
+//
+// Component i is reduced in exactly the scalar order, so it has the same bits as a scalar functor whose terms are
+// component i's terms; the m components cost one map + fold launch pair instead of m.
+//
 // The reduction is deterministic AND independent of the number of ranks: the variables are cut into the library's
 // groups and 8 virtual shards (a function of n alone, nlopt_b200_shard_geometry); one CTA reduces one group with a
 // fixed thread->variable map and a fixed shuffle / shared-memory tree, a second kernel folds the group sums of each
@@ -169,6 +186,80 @@ __global__ void __launch_bounds__(kThreads) fold_groups_kernel(const double *par
     if (threadIdx.x == 0) vsums[blockIdx.x] = s;
 }
 
+// ---- vector functors (nlopt_b200_dmfunc2): F::m components from one visit of each variable ---------------------
+// map_group_mkernel is map_group_kernel with F::m accumulators per thread: the same thread->variable map, every term
+// added with __dadd_rn from +0.0, and each component reduced by block_sum's tree (xor butterfly 16..1, then the 8 warp
+// sums in warp order from +0.0; thread i does the final adds of component i).  So component i ends in the same bits
+// as a scalar functor whose terms are component i's terms.  Group sums go out as [m][groups_local].
+template <class F>
+__global__ void __launch_bounds__(kThreads) map_group_mkernel(F f, nlopt_b200_shard sh, const double *x, double *grad,
+                                                              long long grad_ld, double *partials)
+{
+    constexpr int M = F::m;
+    __shared__ double smem[M][kThreads / 32];
+    const unsigned g = sh.group0 + blockIdx.x;
+    const unsigned long long c_lo = (unsigned long long) g * sh.nchunks / sh.groups_total - sh.chunk0;
+    const unsigned long long c_hi = (unsigned long long) (g + 1) * sh.nchunks / sh.groups_total - sh.chunk0;
+    long long lo = (long long) (c_lo * 512), hi = (long long) (c_hi * 512);
+    if (hi > (long long) sh.n_local) hi = (long long) sh.n_local;
+    double acc[M];
+#pragma unroll
+    for (int i = 0; i < M; ++i) acc[i] = 0.0;
+    for (long long jl = lo + threadIdx.x; jl < hi; jl += kThreads) {
+        double t[M];
+        f(sh.j0 + (unsigned long long) jl, sh.n, jl, (long long) sh.n_local, x, t, grad ? grad + jl : nullptr, grad_ld);
+#pragma unroll
+        for (int i = 0; i < M; ++i) acc[i] = __dadd_rn(acc[i], t[i]);
+    }
+#pragma unroll
+    for (int i = 0; i < M; ++i) {
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) acc[i] = __dadd_rn(acc[i], __shfl_xor_sync(0xffffffffu, acc[i], off));
+    }
+    if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+        for (int i = 0; i < M; ++i) smem[i][threadIdx.x >> 5] = acc[i];
+    }
+    __syncthreads();
+    if (threadIdx.x < M) {
+        double s = 0.0;
+        for (int w = 0; w < kThreads / 32; ++w) s = __dadd_rn(s, smem[threadIdx.x][w]);
+        partials[(size_t) threadIdx.x * gridDim.x + blockIdx.x] = s;
+    }
+}
+
+// fold_groups_kernel for every row: CTA (v, i) folds the P group sums of local virtual shard v of row i in the same
+// fixed order; row i of the partials starts at partials + i * groups_local, of the sums at vsums + 8 i
+__global__ void __launch_bounds__(kThreads) fold_groups_mkernel(const double *partials, unsigned groups_local, unsigned P,
+                                                                double *vsums /* row 0 at vshard0 */)
+{
+    __shared__ double smem[kThreads / 32];
+    const double *base = partials + (size_t) blockIdx.y * groups_local + (size_t) blockIdx.x * P;
+    double acc = 0.0;
+    for (unsigned r = threadIdx.x; r < P; r += kThreads) acc = __dadd_rn(acc, base[r]);
+    const double s = block_sum(acc, smem);
+    if (threadIdx.x == 0) vsums[(size_t) blockIdx.y * 8 + blockIdx.x] = s;
+}
+
+template <class F>
+void mtrampoline2(unsigned /* = F::m, registered by the front ends below */, const nlopt_b200_shard *sh, const double *x_dev,
+                  double *grad_dev, unsigned long long grad_ld, double *vsums_dev, void *data, void *stream)
+{
+    const F *f = static_cast<const F *>(data);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (sh->groups_local == 0) return;
+    double *part = partials2(F::m * sh->groups_local);
+    map_group_mkernel<F><<<sh->groups_local, kThreads, 0, s>>>(*f, *sh, x_dev, grad_dev, (long long) grad_ld, part);
+    fold_groups_mkernel<<<dim3(sh->local_vshards, F::m), kThreads, 0, s>>>(part, sh->groups_local, sh->groups_per_vshard,
+                                                                           vsums_dev + sh->vshard0);
+}
+
+template <class F>
+void mfinish2(unsigned, const double *totals, double *result, void *data)
+{
+    static_cast<const F *>(data)->finish(totals, result);
+}
+
 template <class F, class = void>
 struct halo_of { static constexpr int value = 0; };
 template <class F>
@@ -230,6 +321,24 @@ nlopt_result add_equality_constraint(nlopt_opt opt, const F *f, double tol)
 {
     return nlopt_b200_add_equality_constraint_device2(opt, &detail::trampoline2<F>, &detail::finish2<F>, const_cast<F *>(f), tol,
                                                       detail::halo_of<F>::value);
+}
+
+// F::m constraint rows from one vector functor (one pass over x, one launch pair); tol: F::m doubles or nullptr (zeros)
+template <class F>
+nlopt_result add_inequality_mconstraint(nlopt_opt opt, const F *f, const double *tol)
+{
+    static_assert(F::m >= 1 && F::m <= 16, "a vector functor has 1 to 16 components");
+    return nlopt_b200_add_inequality_mconstraint_device2(opt, F::m, &detail::mtrampoline2<F>, &detail::mfinish2<F>,
+                                                         const_cast<F *>(f), tol, detail::halo_of<F>::value);
+}
+
+// h_i(x) = 0 within tol[i] (the AUGLAG family)
+template <class F>
+nlopt_result add_equality_mconstraint(nlopt_opt opt, const F *f, const double *tol)
+{
+    static_assert(F::m >= 1 && F::m <= 16, "a vector functor has 1 to 16 components");
+    return nlopt_b200_add_equality_mconstraint_device2(opt, F::m, &detail::mtrampoline2<F>, &detail::mfinish2<F>,
+                                                       const_cast<F *>(f), tol, detail::halo_of<F>::value);
 }
 
 // the first form of the interface (one synchronous evaluation per call, nlopt_b200_dfunc), kept for callers that

@@ -189,6 +189,17 @@ class opt:
         self._check(self._lib.nlopt_b200_add_equality_constraint_device(
             self._h, fn_ptr, data_ptr, float(tol)))
 
+    # vector device constraints (nlopt_b200_dmfunc2 / nlopt_b200_dmfinish pointers); m = len(tol)
+    def add_inequality_mconstraint_device(self, fn_ptr, finish_ptr, data_ptr, tol, halo=0):
+        tol = _as_f64(tol)
+        self._check(self._lib.nlopt_b200_add_inequality_mconstraint_device2(
+            self._h, tol.size, fn_ptr, finish_ptr, data_ptr, _ptr(tol), int(halo)))
+
+    def add_equality_mconstraint_device(self, fn_ptr, finish_ptr, data_ptr, tol, halo=0):
+        tol = _as_f64(tol)
+        self._check(self._lib.nlopt_b200_add_equality_mconstraint_device2(
+            self._h, tol.size, fn_ptr, finish_ptr, data_ptr, _ptr(tol), int(halo)))
+
     def optimize_device(self, x_dev_ptr):
         f = C.c_double(0.0)
         self._exc = None

@@ -145,6 +145,10 @@ _EXT = {
     "nlopt_b200_add_equality_constraint_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_double]),
     "nlopt_b200_add_equality_constraint_device2":
         (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_int]),
+    "nlopt_b200_add_inequality_mconstraint_device2":
+        (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p, c_double_p, C.c_int]),
+    "nlopt_b200_add_equality_mconstraint_device2":
+        (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p, c_double_p, C.c_int]),
     "nlopt_b200_shard_geometry": (None, [C.c_ulonglong, C.c_int, C.c_int, C.c_void_p]),
     "nlopt_b200_set_min_objective_sharded": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "nlopt_b200_add_inequality_constraint_sharded": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_double]),

@@ -20,6 +20,8 @@ struct FuncSpec {
     nlopt_b200_dfunc df = nullptr;
     nlopt_b200_dfunc2 df2 = nullptr;         // asynchronous device callback (takes precedence over df) ...
     nlopt_b200_dfinish dfin = nullptr;       // ... and its host-side finish
+    nlopt_b200_dmfunc2 dmf2 = nullptr;       // vector asynchronous device callback, m rows (constraints only) ...
+    nlopt_b200_dmfinish dmfin = nullptr;     // ... and its host-side finish of the m totals
     int halo = 0;
     nlopt_b200_sfunc sf = nullptr;           // sharded host callback
     void *data = nullptr;

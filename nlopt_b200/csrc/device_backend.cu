@@ -653,7 +653,7 @@ bool DeviceBackend::eval_penalty_objective(Slot slot, bool want_grad, double *va
         unsigned row = 0;
         for (int pass = 0; pass < 2; ++pass)
             for (const FuncSpec &fs : (pass == 0 ? ps.eq : ps.ineq)) {
-                if (fs.df2 && !enqueue_df2(fs, slot, want_grad ? pen_rows_ + (size_t) row * geo_.ld : nullptr, 1 + m_ + row))
+                if ((fs.df2 || fs.dmf2) && !enqueue_df2(fs, slot, want_grad ? pen_rows_ + (size_t) row * geo_.ld : nullptr, 1 + m_ + row))
                     return false;
                 row += fs.m;
             }
@@ -670,8 +670,8 @@ bool DeviceBackend::eval_penalty_objective(Slot slot, bool want_grad, double *va
     bool any_partial = false;
     for (int pass = 0; pass < 2; ++pass)
         for (const FuncSpec &fs : (pass == 0 ? ps.eq : ps.ineq)) {
-            if (fs.df2) {
-                vals[row] = settled[m_ + row];
+            if (fs.df2 || fs.dmf2) {
+                for (unsigned r = 0; r < fs.m; ++r) vals[row + r] = settled[m_ + row + r];
             } else if (fs.df) {
                 const double t0 = wall_seconds();
                 vals[row] = fs.df((unsigned) geo_.n_local, geo_.j0, xs, want_grad ? pen_rows_ + (size_t) row * geo_.ld : nullptr, fs.data, stream_);
@@ -788,9 +788,9 @@ bool DeviceBackend::eval_constraint(Slot slot, unsigned ic, unsigned row0, bool 
 {
     const FuncSpec &fs = cfg_.constraints[ic];
     if (fs.sf) return eval_sharded(fs, slot, want_grad ? (slot == kBase ? G_ : Gcur_) + (size_t) row0 * geo_.ld : nullptr, 1 + row0, values);
-    if (fs.df2) {
+    if (fs.df2 || fs.dmf2) {
         double *gs = want_grad ? (slot == kBase ? G_ : Gcur_) + (size_t) row0 * geo_.ld : nullptr;
-        values[0] = 0.0;
+        for (unsigned r = 0; r < fs.m; ++r) values[r] = 0.0;
         return enqueue_df2(fs, slot, gs, 1 + row0);
     }
     if (fs.df) {
@@ -858,7 +858,8 @@ bool DeviceBackend::eval_sharded(const FuncSpec &fs, Slot slot, double *grad_dst
     return true;
 }
 
-// Asynchronous device callbacks (nlopt_b200_dfunc2): enqueue, remember which value is pending.
+// Asynchronous device callbacks (nlopt_b200_dfunc2): enqueue, remember which value is pending.  A vector callback
+// (nlopt_b200_dmfunc2) takes the m slots [index, index + m) and the m gradient rows from grad_dst on, stride ld.
 bool DeviceBackend::enqueue_df2(const FuncSpec &fs, Slot slot, double *grad_dst, unsigned index)
 {
     Comm &comm = Comm::instance();
@@ -877,10 +878,11 @@ bool DeviceBackend::enqueue_df2(const FuncSpec &fs, Slot slot, double *grad_dst,
     if (fs.halo > 0 && !ensure_halo(slot)) return false;
     double *xs = slot == kBase ? x_ : xcur_view();
     const double t0 = wall_seconds();
-    fs.df2(&shard_, xs, grad_dst, vs2_dev_ + (size_t) index * kV, fs.data, stream_);
+    if (fs.dmf2) fs.dmf2(fs.m, &shard_, xs, grad_dst, geo_.ld, vs2_dev_ + (size_t) index * kV, fs.data, stream_);
+    else fs.df2(&shard_, xs, grad_dst, vs2_dev_ + (size_t) index * kV, fs.data, stream_);
     cb_seconds_ += wall_seconds() - t0;
     NB_CUDA(cudaGetLastError());
-    pend2_[index] = &fs;
+    for (unsigned r = 0; r < fs.m; ++r) pend2_[index + r] = &fs;
     pend2_any_ = true;
     return true;
 }
@@ -924,9 +926,25 @@ bool DeviceBackend::finish_evals(double *fvalue, double *cvalues)
         if (comm.active() && comm.all_reduce_sum(vs2_dev_, vs2_cap_ * kV, stream_, &err_)) return false;
         NB_CUDA(cudaMemcpyAsync(vs2_host_, vs2_dev_, vs2_cap_ * kV * sizeof(double), cudaMemcpyDeviceToHost, stream_));
         NB_CUDA(cudaStreamSynchronize(stream_));
-        for (size_t i = 0; i < vs2_cap_; ++i) {
+        size_t step = 1;
+        for (size_t i = 0; i < vs2_cap_; i += step) {
             const FuncSpec *fs = pend2_[i];
+            step = 1;
             if (!fs) continue;
+            if (fs->dmf2) {            // a vector constraint: its m rows, one finish call (never the objective's slot 0)
+                step = fs->m;
+                if (!cvalues) continue;
+                std::vector<double> tots(fs->m);
+                for (unsigned r = 0; r < fs->m; ++r) {
+                    const double *vs = vs2_host_ + (i + r) * kV;
+                    double tot = vs[0];
+                    for (unsigned v = 1; v < kV; ++v) tot += vs[v];
+                    tots[r] = tot;
+                }
+                fs->dmfin(fs->m, tots.data(), cvalues + i - 1, fs->data);
+                for (unsigned r = 0; r < fs->m; ++r) pend2_[i + r] = nullptr;
+                continue;
+            }
             double tot = vs2_host_[i * kV];
             for (unsigned v = 1; v < kV; ++v) tot += vs2_host_[i * kV + v];
             const double val = fs->dfin(tot, fs->data);

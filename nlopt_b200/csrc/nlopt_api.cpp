@@ -84,11 +84,13 @@ void munge_all(nlopt_opt o, std::vector<ConstraintRec> &v)
 }
 
 // options.c:504-547
+// vector_form: dfc is the marker of a vector device callback (nlopt_b200_add_*_mconstraint_device2), any fm
 nlopt_result add_constraint(nlopt_opt opt, std::vector<ConstraintRec> &list, unsigned fm, nlopt_func fc,
-                            nlopt_mfunc mfc, nlopt_b200_dfunc dfc, nlopt_precond pre, void *data, const double *tol)
+                            nlopt_mfunc mfc, nlopt_b200_dfunc dfc, nlopt_precond pre, void *data, const double *tol,
+                            bool vector_form)
 {
     const int kinds = (fc != nullptr) + (mfc != nullptr) + (dfc != nullptr);
-    if (kinds != 1 || ((fc || dfc) && fm != 1)) return NLOPT_INVALID_ARGS;
+    if (kinds != 1 || ((fc || (dfc && !vector_form)) && fm != 1)) return NLOPT_INVALID_ARGS;
     if (tol)
         for (unsigned i = 0; i < fm; ++i)
             if (tol[i] < 0) { set_err(opt, "negative constraint tolerance"); return NLOPT_INVALID_ARGS; }
@@ -500,7 +502,7 @@ static nlopt_result add_any(nlopt_opt opt, bool equality, bool vector_form, unsi
         set_err(opt, "invalid algorithm for constraints");
         ret = NLOPT_INVALID_ARGS;
     } else
-        ret = add_constraint(opt, equality ? opt->h : opt->fc, m, fc, mfc, dfc, pre, data, tol);
+        ret = add_constraint(opt, equality ? opt->h : opt->fc, m, fc, mfc, dfc, pre, data, tol, vector_form);
     if (ret < 0 && opt && opt->munge_on_destroy) opt->munge_on_destroy(data);
     return ret;
 }
@@ -553,6 +555,27 @@ nlopt_result nlopt_b200_add_equality_constraint_device2(nlopt_opt opt, nlopt_b20
     c.halo = halo;
     return r;
 }
+
+// the vector twins: registered like nlopt_add_*_mconstraint (m == 0 is accepted and registers nothing), with the
+// scalar _device2 argument checks and the marker in df
+static nlopt_result add_device_m(nlopt_opt opt, bool equality, unsigned m, nlopt_b200_dmfunc2 fc, nlopt_b200_dmfinish fin,
+                                 void *d, const double *tol, int halo)
+{
+    if (m && (!fc || !fin || halo < 0 || halo > 1)) return NLOPT_INVALID_ARGS;
+    nlopt_result r = add_any(opt, equality, true, m, nullptr, nullptr, df2_marker, nullptr, d, tol);
+    if (r < 0 || !m) return r;
+    nb200::ConstraintRec &c = (equality ? opt->h : opt->fc).back();
+    c.dmf2 = fc;
+    c.dmfin = fin;
+    c.halo = halo;
+    return r;
+}
+nlopt_result nlopt_b200_add_inequality_mconstraint_device2(nlopt_opt opt, unsigned m, nlopt_b200_dmfunc2 fc,
+                                                           nlopt_b200_dmfinish fin, void *d, const double *tol, int halo)
+{ return add_device_m(opt, false, m, fc, fin, d, tol, halo); }
+nlopt_result nlopt_b200_add_equality_mconstraint_device2(nlopt_opt opt, unsigned m, nlopt_b200_dmfunc2 h,
+                                                         nlopt_b200_dmfinish fin, void *d, const double *tol, int halo)
+{ return add_device_m(opt, true, m, h, fin, d, tol, halo); }
 
 /* ------------------------------------------------------------------ stopping criteria (options.c:661-816) */
 
@@ -941,7 +964,9 @@ nlopt_result run_ccsa(nlopt_opt opt, double *x_host, double *x_dev, double *minf
     bool any_pre = opt->pre != nullptr;
     for (const auto &c : opt->fc) any_pre = any_pre || c.pre != nullptr;
     if (any_pre && opt->algorithm == NLOPT_LD_CCSAQ) {          /* ccsa_quadratic.c: the !no_precond branch */
-        if (!x_host || opt->df) {
+        bool dev_c = false;                                     /* device (scalar or vector) or sharded constraints */
+        for (const auto &c : opt->fc) dev_c = dev_c || c.df;
+        if (!x_host || opt->df || dev_c) {
             set_err(opt, "preconditioned CCSAQ takes host x and host callbacks (nlopt_precond is a host function)");
             return NLOPT_INVALID_ARGS;
         }
@@ -963,7 +988,8 @@ nlopt_result run_ccsa(nlopt_opt opt, double *x_host, double *x_dev, double *minf
     std::vector<double> tol;
     for (const auto &c : opt->fc) {
         nb200::FuncSpec s;
-        s.m = c.m; s.f = c.f; s.mf = c.mf; s.df = c.df; s.df2 = c.df2; s.dfin = c.dfin; s.halo = c.halo; s.sf = c.sf; s.data = c.f_data;
+        s.m = c.m; s.f = c.f; s.mf = c.mf; s.df = c.df; s.df2 = c.df2; s.dfin = c.dfin; s.dmf2 = c.dmf2; s.dmfin = c.dmfin;
+        s.halo = c.halo; s.sf = c.sf; s.data = c.f_data;
         cfg.constraints.push_back(s);
         tol.insert(tol.end(), c.tol.begin(), c.tol.end());
     }
@@ -1406,7 +1432,8 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
     std::vector<double> lambda(pp ? pp : 1, 0.0), mu(mm ? mm : 1, 0.0);
     auto to_spec = [](const nb200::ConstraintRec &c) {
         nb200::FuncSpec s;
-        s.m = c.m; s.f = c.f; s.mf = c.mf; s.df = c.df; s.df2 = c.df2; s.dfin = c.dfin; s.halo = c.halo; s.data = c.f_data;
+        s.m = c.m; s.f = c.f; s.mf = c.mf; s.df = c.df; s.df2 = c.df2; s.dfin = c.dfin; s.dmf2 = c.dmf2; s.dmfin = c.dmfin;
+        s.halo = c.halo; s.data = c.f_data;
         return s;
     };
     for (const auto &c : opt->h) pen.eq.push_back(to_spec(c));
@@ -1443,7 +1470,8 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
         sub->munge_on_copy = mc;
     }
     for (const auto &c : sub_fc) {
-        nlopt_result r = c.df2 ? nlopt_b200_add_inequality_constraint_device2(sub, c.df2, c.dfin, c.f_data, c.tol[0], c.halo)
+        nlopt_result r = c.dmf2 ? nlopt_b200_add_inequality_mconstraint_device2(sub, c.m, c.dmf2, c.dmfin, c.f_data, c.tol.data(), c.halo)
+                       : c.df2 ? nlopt_b200_add_inequality_constraint_device2(sub, c.df2, c.dfin, c.f_data, c.tol[0], c.halo)
                        : c.df  ? nlopt_b200_add_inequality_constraint_device(sub, c.df, c.f_data, c.tol[0])
                        : c.f   ? nlopt_add_inequality_constraint(sub, c.f, c.f_data, c.tol[0])
                                : nlopt_add_inequality_mconstraint(sub, c.m, c.mf, c.f_data, c.tol.data());

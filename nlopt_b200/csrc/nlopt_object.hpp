@@ -20,6 +20,8 @@ struct ConstraintRec {
     nlopt_b200_dfunc df = nullptr;  // scalar device callback (extension)
     nlopt_b200_dfunc2 df2 = nullptr;    // asynchronous form (df then holds a marker)
     nlopt_b200_dfinish dfin = nullptr;
+    nlopt_b200_dmfunc2 dmf2 = nullptr;  // vector asynchronous form, m rows (df then holds a marker)
+    nlopt_b200_dmfinish dmfin = nullptr;
     int halo = 0;
     nlopt_b200_sfunc sf = nullptr;      // sharded host callback (df then holds a marker)
     nlopt_precond pre = nullptr;

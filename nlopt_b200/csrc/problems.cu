@@ -14,6 +14,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <vector>
 
 #include "../../include/nlopt_b200_device.cuh"
@@ -126,6 +127,76 @@ int add_eq(nlopt_opt opt, const F *f, double tol, int sync)
     return sync ? nlopt_b200::add_equality_constraint_sync(opt, f, tol) : nlopt_b200::add_equality_constraint(opt, f, tol);
 }
 
+// ---- vector functors (one pass over x for M constraint rows) ---------------------------------------------
+// M dense linear rows c_i(x) = w_i.x - b_i: the one-functor form of M LinearDev.  Component i has LinearDev's terms
+// w_ij * x_j, so it has the same bits as LinearDev with row w_i.
+template <int M>
+struct LinearRowsDev {
+    static constexpr int m = M;
+    const double *w;        // device, [M][w_ld]: this rank's shard of each weight row
+    long long w_ld;
+    double b[M];
+    __device__ void operator()(unsigned long long, unsigned long long, long long jl, long long, const double *x, double *t,
+                               double *grad, long long grad_ld) const
+    {
+        const double xj = x[jl];
+#pragma unroll
+        for (int i = 0; i < M; ++i) {
+            const double wij = w[i * w_ld + jl];
+            if (grad) grad[i * grad_ld] = wij;
+            t[i] = __dmul_rn(wij, xj);
+        }
+    }
+    void finish(const double *s, double *c) const
+    {
+        for (int i = 0; i < M; ++i) c[i] = s[i] - b[i];
+    }
+};
+
+// local volumes: c_i(x) = mean of x over the block [i n / M, (i + 1) n / M) - target_i.  Component i's term is x_j
+// inside block i and +0.0 outside; its gradient 1 / |block i| inside and 0 outside.
+template <int M>
+struct BlockMeanDev {
+    static constexpr int m = M;
+    unsigned long long edge[M + 1];     // block i = [edge[i], edge[i + 1])
+    double inv_len[M], target[M];
+    __device__ void operator()(unsigned long long j, unsigned long long, long long jl, long long, const double *x, double *t,
+                               double *grad, long long grad_ld) const
+    {
+        const double xj = x[jl];
+#pragma unroll
+        for (int i = 0; i < M; ++i) {
+            const bool in = j >= edge[i] && j < edge[i + 1];
+            if (grad) grad[i * grad_ld] = in ? inv_len[i] : 0.0;
+            t[i] = in ? xj : 0.0;
+        }
+    }
+    void finish(const double *s, double *c) const
+    {
+        for (int i = 0; i < M; ++i) c[i] = s[i] * inv_len[i] - target[i];
+    }
+};
+
+// Op<M>::run(args...) for M in {1, 2, 4, 8, 16}
+template <template <int> class Op, class... A>
+int with_m(unsigned m, A... a)
+{
+    switch (m) {
+    case 1: return Op<1>::run(a...);
+    case 2: return Op<2>::run(a...);
+    case 4: return Op<4>::run(a...);
+    case 8: return Op<8>::run(a...);
+    case 16: return Op<16>::run(a...);
+    default: return NLOPT_INVALID_ARGS;
+    }
+}
+
+template <class F>
+int add_m(nlopt_opt opt, const F *f, const double *tol, int equality)
+{
+    return equality ? nlopt_b200::add_equality_mconstraint(opt, f, tol) : nlopt_b200::add_inequality_mconstraint(opt, f, tol);
+}
+
 }  // namespace
 
 struct nb200p_lin_data {
@@ -153,7 +224,51 @@ struct nb200p_problem_s {
     std::vector<nb200p_lin_data *> lin_host;
     SimpDev simp;
     std::vector<void *> misc_host;          // small data records of the host callbacks (freed with the problem)
+    std::vector<std::shared_ptr<void>> vec; // vector functors (LinearRowsDev<M>, BlockMeanDev<M>)
 };
+
+namespace {
+
+template <int M>
+struct AddLinearRows {
+    // w_host: [M][n] row-major, b: M offsets
+    static int run(nb200p_problem_s *p, nlopt_opt opt, const double *w_host, const double *b, const double *tol, int equality)
+    {
+        const unsigned n = nlopt_get_dimension(opt);
+        unsigned long long j0 = 0, cnt = n;
+        nlopt_b200_shard_range(n, nlopt_b200_comm_rank(), nlopt_b200_comm_world(), &j0, &cnt);
+        double *w = nullptr;
+        if (cudaMalloc(&w, (size_t) M * (cnt ? cnt : 1) * sizeof(double)) != cudaSuccess) return NLOPT_OUT_OF_MEMORY;
+        p->dev_rows.push_back(w);
+        if (cnt && cudaMemcpy2D(w, cnt * sizeof(double), w_host + j0, (size_t) n * sizeof(double), cnt * sizeof(double), M,
+                                cudaMemcpyHostToDevice) != cudaSuccess)
+            return NLOPT_FAILURE;
+        auto f = std::make_shared<LinearRowsDev<M>>();
+        f->w = w;
+        f->w_ld = (long long) cnt;
+        for (int i = 0; i < M; ++i) f->b[i] = b[i];
+        p->vec.push_back(f);
+        return add_m(opt, f.get(), tol, equality);
+    }
+};
+
+template <int M>
+struct AddBlockMean {
+    static int run(nb200p_problem_s *p, nlopt_opt opt, const double *target, const double *tol, int equality)
+    {
+        const unsigned long long n = nlopt_get_dimension(opt);
+        auto f = std::make_shared<BlockMeanDev<M>>();
+        for (int i = 0; i <= M; ++i) f->edge[i] = (unsigned long long) i * n / M;
+        for (int i = 0; i < M; ++i) {
+            f->inv_len[i] = 1.0 / (double) (f->edge[i + 1] - f->edge[i]);
+            f->target[i] = target[i];
+        }
+        p->vec.push_back(f);
+        return add_m(opt, f.get(), tol, equality);
+    }
+};
+
+}  // namespace
 
 extern "C" {
 
@@ -219,6 +334,21 @@ int nb200p_add_sphere_device_eq(nb200p_problem_s *p, nlopt_opt opt, double r, do
     SphereDev *s = new SphereDev{1.0 / (double) nlopt_get_dimension(opt), r};
     p->sphere.push_back(s);
     return add_eq(opt, s, tol, sync);
+}
+
+// vector constraints, m in {1, 2, 4, 8, 16}; equality != 0 registers h(x) = 0 (NLOPT_AUGLAG*).  tol: m entries or NULL.
+// m dense linear rows w_k.x - b_k, w_host_rows [m][n] row-major (copied to the device here)
+int nb200p_add_linear_rows_device(nb200p_problem_s *p, nlopt_opt opt, unsigned m, const double *w_host_rows, const double *b,
+                                  const double *tol, int equality)
+{
+    return with_m<AddLinearRows>(m, p, opt, w_host_rows, b, tol, equality);
+}
+
+// block means: c_i = mean(x over [i n / m, (i + 1) n / m)) - target_i
+int nb200p_add_block_mean_device(nb200p_problem_s *p, nlopt_opt opt, unsigned m, const double *target, const double *tol,
+                                 int equality)
+{
+    return with_m<AddBlockMean>(m, p, opt, target, tol, equality);
 }
 
 // the synchronous forms of the quadratic / SIMP objectives and the mean inequality

@@ -32,6 +32,8 @@ def _load():
     L.nb200p_set_quadratic_device_sync.argtypes = [C.c_void_p, C.c_void_p, C.c_ulonglong]
     L.nb200p_set_simp_device_sync.argtypes = [C.c_void_p, C.c_void_p, C.c_ulonglong, C.c_double]
     L.nb200p_add_mean_device_sync.argtypes = [C.c_void_p, C.c_void_p, C.c_double, C.c_double]
+    L.nb200p_add_linear_rows_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint, c_double_p, c_double_p, c_double_p, C.c_int]
+    L.nb200p_add_block_mean_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint, c_double_p, c_double_p, C.c_int]
     for nm, args in (("nb200p_make_simp_data", [C.c_void_p, C.c_ulonglong, C.c_double]),
                      ("nb200p_make_mean_data", [C.c_void_p, C.c_double]), ("nb200p_make_quad_data", [C.c_void_p, C.c_ulonglong])):
         getattr(L, nm).restype = C.c_void_p
@@ -79,6 +81,38 @@ class Problem:
         for k in range(m):
             w = linear_weights(k, n)
             opt._check(self.L.nb200p_add_linear_device(self.h, opt._h, w.ctypes.data_as(c_double_p), 0.5 + 0.1 * k, tol))
+
+    # ---- vector device constraints: m rows from one functor, m in {1, 2, 4, 8, 16} ----
+    def add_linear_rows_device(self, opt, w, b, tol=0.0, equality=False):
+        """m dense linear rows  w_k.x - b_k  (<= 0, or = 0 with equality=True); w: [m][n]"""
+        w = np.ascontiguousarray(w, dtype=np.float64)
+        m = w.shape[0]
+        b = np.ascontiguousarray(np.broadcast_to(b, (m,)), dtype=np.float64)
+        tol = np.ascontiguousarray(np.broadcast_to(tol, (m,)), dtype=np.float64)
+        opt._check(self.L.nb200p_add_linear_rows_device(self.h, opt._h, m, w.ctypes.data_as(c_double_p),
+                                                        b.ctypes.data_as(c_double_p), tol.ctypes.data_as(c_double_p), int(equality)))
+
+    def rosenbrock_device_rows(self, opt, m, tol=1e-8):
+        """rosenbrock_device with its m LinearDev rows as one LinearRowsDev<m>: the same weights and offsets"""
+        n = opt.get_dimension()
+        opt._check(self.L.nb200p_set_rosenbrock_device(self.h, opt._h))
+        if m:
+            self.add_linear_rows_device(opt, np.stack([linear_weights(k, n) for k in range(m)]),
+                                        [0.5 + 0.1 * k for k in range(m)], tol)
+
+    def add_block_mean_device(self, opt, targets, tol=0.0):
+        """local volumes  mean(x over block i) - targets[i] <= 0, block i = [i n / m, (i + 1) n / m)"""
+        self._block_mean(opt, targets, tol, False)
+
+    def add_block_mean_device_eq(self, opt, targets, tol=0.0):
+        """local volumes as equalities (NLOPT_AUGLAG*)"""
+        self._block_mean(opt, targets, tol, True)
+
+    def _block_mean(self, opt, targets, tol, equality):
+        t = np.ascontiguousarray(targets, dtype=np.float64)
+        tol = np.ascontiguousarray(np.broadcast_to(tol, t.shape), dtype=np.float64)
+        opt._check(self.L.nb200p_add_block_mean_device(self.h, opt._h, t.size, t.ctypes.data_as(c_double_p),
+                                                       tol.ctypes.data_as(c_double_p), int(equality)))
 
     def quadratic_device(self, opt, seed=0x5EED0000, offset=0.1, tol=0.0):
         opt._check(self.L.nb200p_set_quadratic_device(self.h, opt._h, seed))
