@@ -19,9 +19,13 @@
  * equality constraints, either form) and nlopt_b200_optimize_device as
  * well; host and device callbacks may be mixed.  Such a run keeps x and its
  * best point in HBM and evaluates the outer loop's values on the device
- * (one GPU only; sharded host callbacks and maximisation with a device
- * objective are refused).  After any AUGLAG run nlopt_b200_get_stats
- * reports the last sub-optimisation.
+ * (one GPU only; sharded host callbacks are refused).  After any AUGLAG run
+ * nlopt_b200_get_stats reports the last sub-optimisation.
+ *
+ * Maximisation works with every objective form: nlopt_set_max_objective for
+ * host callbacks and the nlopt_b200_set_max_objective_* twins of the device
+ * and sharded entry points, under LD_MMA, LD_CCSAQ and the AUGLAG family
+ * (sharded objectives under LD_MMA / LD_CCSAQ only).
  *
  * The `nlopt_b200_*` symbols are additive extensions (device-resident
  * callbacks, kernel-level access to the dual evaluation, multi-GPU sharding,
@@ -220,6 +224,12 @@ void nlopt_set_stochastic_population(int pop);
 typedef double (*nlopt_b200_dfunc)(unsigned n_local, unsigned long long j0, const double *x_dev,
                                    double *grad_dev, void *func_data, void *cuda_stream);
 nlopt_result nlopt_b200_set_min_objective_device(nlopt_opt opt, nlopt_b200_dfunc f, void *f_data);
+/* Maximisation (the device twins of nlopt_set_max_objective, here and for the forms below): the callback returns f and
+ * writes grad f of the function to MAXIMISE; the library minimises -f and reports opt_f = f.  The sign flip is exact:
+ * the value is negated once it is final (after the sum over ranks and finish) and the gradient by one kernel on the
+ * library stream right after the callback, so a maximisation of -F runs through the same points as a minimisation of F,
+ * bit for bit (as long as no sum of terms is exactly zero, whose sign may differ).  Argument checks and the stopval handling are those of the _min_ form / nlopt_set_max_objective. */
+nlopt_result nlopt_b200_set_max_objective_device(nlopt_opt opt, nlopt_b200_dfunc f, void *f_data);
 nlopt_result nlopt_b200_add_inequality_constraint_device(nlopt_opt opt, nlopt_b200_dfunc fc,
                                                          void *fc_data, double tol);
 /* h(x) = 0 within tol: accepted by the algorithms that take nlopt_add_equality_constraint (the AUGLAG family here);
@@ -249,6 +259,9 @@ typedef void (*nlopt_b200_dfunc2)(const nlopt_b200_shard *shard, const double *x
                                   void *func_data, void *cuda_stream);
 typedef double (*nlopt_b200_dfinish)(double total, void *func_data);
 nlopt_result nlopt_b200_set_min_objective_device2(nlopt_opt opt, nlopt_b200_dfunc2 f, nlopt_b200_dfinish finish,
+                                                  void *f_data, int halo);
+/* maximise: finish(total) is the value of the function to maximise (see nlopt_b200_set_max_objective_device) */
+nlopt_result nlopt_b200_set_max_objective_device2(nlopt_opt opt, nlopt_b200_dfunc2 f, nlopt_b200_dfinish finish,
                                                   void *f_data, int halo);
 nlopt_result nlopt_b200_add_inequality_constraint_device2(nlopt_opt opt, nlopt_b200_dfunc2 fc, nlopt_b200_dfinish finish,
                                                           void *fc_data, double tol, int halo);
@@ -283,6 +296,8 @@ nlopt_result nlopt_b200_add_equality_mconstraint_device2(nlopt_opt opt, unsigned
 typedef double (*nlopt_b200_sfunc)(unsigned n_local, unsigned long long j0, unsigned long long n, const double *x_shard,
                                    double *grad_shard, void *func_data);
 nlopt_result nlopt_b200_set_min_objective_sharded(nlopt_opt opt, nlopt_b200_sfunc f, void *f_data);
+/* maximise (LD_MMA / LD_CCSAQ; see nlopt_b200_set_max_objective_device) */
+nlopt_result nlopt_b200_set_max_objective_sharded(nlopt_opt opt, nlopt_b200_sfunc f, void *f_data);
 nlopt_result nlopt_b200_add_inequality_constraint_sharded(nlopt_opt opt, nlopt_b200_sfunc fc, void *fc_data, double tol);
 /* like nlopt_optimize, but x_dev is a device array of this rank's shard (in/out) */
 nlopt_result nlopt_b200_optimize_device(nlopt_opt opt, double *x_dev, double *opt_f);

@@ -23,6 +23,7 @@
 //   };
 //
 // Usage:   nlopt_b200::set_min_objective(opt, &functor);     // functor must outlive opt
+//          nlopt_b200::set_max_objective(opt, &functor);     // maximise: the library negates value and gradient
 //          nlopt_b200::add_inequality_constraint(opt, &cfunctor, tol);
 //          nlopt_b200::add_equality_constraint(opt, &hfunctor, tol);      // NLOPT_AUGLAG* only
 //
@@ -308,6 +309,14 @@ nlopt_result set_min_objective(nlopt_opt opt, const F *f)
                                                 detail::halo_of<F>::value);
 }
 
+// maximise F (nlopt_b200_set_max_objective_device2): the library minimises -F and reports opt_f = F at the optimum
+template <class F>
+nlopt_result set_max_objective(nlopt_opt opt, const F *f)
+{
+    return nlopt_b200_set_max_objective_device2(opt, &detail::trampoline2<F>, &detail::finish2<F>, const_cast<F *>(f),
+                                                detail::halo_of<F>::value);
+}
+
 template <class F>
 nlopt_result add_inequality_constraint(nlopt_opt opt, const F *f, double tol)
 {
@@ -348,6 +357,13 @@ nlopt_result set_min_objective_sync(nlopt_opt opt, const F *f)
 {
     auto *b = new detail::Bound<F>{f, nlopt_get_dimension(opt)};      // lives as long as the process
     return nlopt_b200_set_min_objective_device(opt, &detail::trampoline<F>, b);
+}
+
+template <class F>
+nlopt_result set_max_objective_sync(nlopt_opt opt, const F *f)
+{
+    auto *b = new detail::Bound<F>{f, nlopt_get_dimension(opt)};      // lives as long as the process
+    return nlopt_b200_set_max_objective_device(opt, &detail::trampoline<F>, b);
 }
 
 template <class F>

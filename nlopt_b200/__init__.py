@@ -181,6 +181,17 @@ class opt:
     def set_min_objective_device(self, fn_ptr, data_ptr=None):
         self._check(self._lib.nlopt_b200_set_min_objective_device(self._h, fn_ptr, data_ptr))
 
+    def set_max_objective_device(self, fn_ptr, data_ptr=None):
+        """maximise the function of an nlopt_b200_dfunc pointer: the library minimises its negation"""
+        self._check(self._lib.nlopt_b200_set_max_objective_device(self._h, fn_ptr, data_ptr))
+
+    # asynchronous device objectives (nlopt_b200_dfunc2 / nlopt_b200_dfinish pointers)
+    def set_min_objective_device2(self, fn_ptr, finish_ptr, data_ptr=None, halo=0):
+        self._check(self._lib.nlopt_b200_set_min_objective_device2(self._h, fn_ptr, finish_ptr, data_ptr, int(halo)))
+
+    def set_max_objective_device2(self, fn_ptr, finish_ptr, data_ptr=None, halo=0):
+        self._check(self._lib.nlopt_b200_set_max_objective_device2(self._h, fn_ptr, finish_ptr, data_ptr, int(halo)))
+
     def add_inequality_constraint_device(self, fn_ptr, data_ptr=None, tol=0.0):
         self._check(self._lib.nlopt_b200_add_inequality_constraint_device(
             self._h, fn_ptr, data_ptr, float(tol)))

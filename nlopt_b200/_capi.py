@@ -140,6 +140,9 @@ _EXT = {
     "nlopt_b200_add_inequality_constraint_device":
         (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_double]),
     "nlopt_b200_set_min_objective_device2": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
+    "nlopt_b200_set_max_objective_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "nlopt_b200_set_max_objective_device2": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
+    "nlopt_b200_set_max_objective_sharded": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "nlopt_b200_add_inequality_constraint_device2":
         (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_int]),
     "nlopt_b200_add_equality_constraint_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_double]),

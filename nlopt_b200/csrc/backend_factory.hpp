@@ -25,6 +25,8 @@ struct FuncSpec {
     int halo = 0;
     nlopt_b200_sfunc sf = nullptr;           // sharded host callback
     void *data = nullptr;
+    bool negate = false;                     // objective of a maximisation (device / sharded callbacks only): the
+                                             // backend minimises -f -- final value and gradient change sign
 };
 
 // The augmented-Lagrangian objective of NLOPT_AUGLAG* (src/algs/auglag/auglag.c:25-65), evaluated by the backend:

@@ -10,6 +10,7 @@
 //   end_outer_kernel      : nlopt_stop_x norms (src/util/stop.c:98-108) + sigma update (mma.c:431-442,
 //                           ccsa_quadratic.c:577-590) + xprev/xprevprev rotation (mma.c:264-265), one pass
 //   penalty_axpy_kernel   : gradient of the augmented-Lagrangian objective (src/algs/auglag/auglag.c:47-48, :59-60)
+//   negate_kernel         : sign flip of a maximised device / sharded objective's gradient (optimize.c:969-989)
 //
 // Arithmetic contract: every per-variable expression is evaluated with the reference's operation
 // order using __dmul_rn/__dadd_rn/__dsub_rn/__ddiv_rn/__dsqrt_rn, which nvcc never contracts into
@@ -2249,6 +2250,29 @@ __global__ void __launch_bounds__(kBlock) penalty_axpy_kernel(double *__restrict
         double v = g[j];
         for (int k = 0; k < pc.count; ++k) v = addx(v, mulx(pc.c[k], rows[(unsigned long long) pc.row[k] * ld + j]));
         g[j] = v;
+    }
+}
+
+// Maximisation with a device or sharded objective (nlopt_b200_set_max_objective_*): the library minimises -f, so the
+// gradient the callback wrote is negated in place.  Flipping the sign bit is IEEE negation and gives the bits of
+// g[j] = -g[j] on the host for every input: +-0, subnormals, infinities and NaN payloads only change sign.  Two
+// variables per 128-bit load and store (a row starts 16-byte aligned); an odd n_local leaves one tail element.  Exactly
+// n_local entries are touched: the padding lanes stay +0.0.
+__global__ void __launch_bounds__(kBlock) negate_kernel(double *__restrict__ g, unsigned long long n_local)
+{
+    constexpr unsigned long long kSign = 0x8000000000000000ull;
+    const unsigned long long pairs = n_local >> 1, stride = (unsigned long long) gridDim.x * blockDim.x;
+    const unsigned long long t = (unsigned long long) blockIdx.x * blockDim.x + threadIdx.x;
+    ulonglong2 *g2 = reinterpret_cast<ulonglong2 *>(g);
+    for (unsigned long long p = t; p < pairs; p += stride) {
+        ulonglong2 v = g2[p];
+        v.x ^= kSign;
+        v.y ^= kSign;
+        g2[p] = v;
+    }
+    if ((n_local & 1) && t == 0) {
+        unsigned long long *tail = reinterpret_cast<unsigned long long *>(g) + (n_local - 1);
+        *tail ^= kSign;
     }
 }
 

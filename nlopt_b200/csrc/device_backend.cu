@@ -751,14 +751,33 @@ bool DeviceBackend::push_rows_to(double *dst, unsigned rows, const double *host_
     return true;
 }
 
+// A maximised device or sharded objective (FuncSpec::negate): the gradient the callback has just written or enqueued on
+// the library stream changes sign in place, in stream order before any kernel that reads it.
+bool DeviceBackend::negate_gradient(double *g)
+{
+    if (!g || geo_.n_local == 0) return true;
+    negate_kernel<<<grid_for((geo_.n_local + 1) / 2, sm_count_), kBlock, 0, stream_>>>(g, geo_.n_local);
+    ++stats_->kernel_launches;
+    NB_CUDA(cudaGetLastError());
+    return true;
+}
+
+// With FuncSpec::negate the objective's value changes sign once it is final: here for one rank, in finish_evals() for
+// shard contributions and for the asynchronous form.
 bool DeviceBackend::eval_user_objective(Slot slot, bool want_grad, double *value)
 {
     const FuncSpec &fs = cfg_.objective;
-    if (fs.sf) return eval_sharded(fs, slot, want_grad ? (slot == kBase ? g_ : gcur_) : nullptr, 0, value);
+    if (fs.sf) {
+        double *gs = want_grad ? (slot == kBase ? g_ : gcur_) : nullptr;
+        if (!eval_sharded(fs, slot, gs, 0, value)) return false;
+        if (fs.negate && !Comm::instance().active()) *value = -*value;
+        return !fs.negate || negate_gradient(gs);
+    }
     if (fs.df2) {
         double *gs = want_grad ? (slot == kBase ? g_ : gcur_) : nullptr;
         *value = 0.0;                                  // settled in finish_evals()
-        return enqueue_df2(fs, slot, gs, 0);
+        if (!enqueue_df2(fs, slot, gs, 0)) return false;
+        return !fs.negate || negate_gradient(gs);
     }
     if (fs.df) {
         double *xs = slot == kBase ? x_ : xcur_view();
@@ -770,9 +789,10 @@ bool DeviceBackend::eval_user_objective(Slot slot, bool want_grad, double *value
             pend_val_[0] = v;
             pend_set_[0] = 1;
             pend_any_ = true;
-        }
+        } else if (fs.negate)
+            v = -v;
         *value = v;
-        return true;
+        return !fs.negate || negate_gradient(gs);
     }
     if (!fs.f) return fail("no objective function");
     if (!host_x_for(slot)) return false;
@@ -948,7 +968,7 @@ bool DeviceBackend::finish_evals(double *fvalue, double *cvalues)
             double tot = vs2_host_[i * kV];
             for (unsigned v = 1; v < kV; ++v) tot += vs2_host_[i * kV + v];
             const double val = fs->dfin(tot, fs->data);
-            if (i == 0) { if (fvalue) *fvalue = val; else continue; }
+            if (i == 0) { if (fvalue) *fvalue = fs->negate ? -val : val; else continue; }
             else { if (cvalues) cvalues[i - 1] = val; else continue; }
             pend2_[i] = nullptr;
         }
@@ -970,7 +990,7 @@ bool DeviceBackend::finish_evals(double *fvalue, double *cvalues)
     if (comm.all_reduce_sum(scalar_dev_, cnt, stream_, &err_)) return false;
     NB_CUDA(cudaMemcpyAsync(buf.data(), scalar_dev_, cnt * sizeof(double), cudaMemcpyDeviceToHost, stream_));
     NB_CUDA(cudaStreamSynchronize(stream_));
-    if (fvalue && pend_set_[0]) { *fvalue = buf[0]; pend_set_[0] = 0; }
+    if (fvalue && pend_set_[0]) { *fvalue = cfg_.objective.negate ? -buf[0] : buf[0]; pend_set_[0] = 0; }
     if (cvalues)
         for (unsigned i = 0; i < m_; ++i)
             if (pend_set_[1 + i]) { cvalues[i] = buf[1 + i]; pend_set_[1 + i] = 0; }

@@ -50,6 +50,7 @@ public:
     bool ensure_halo(Slot slot);
     bool eval_sharded(const FuncSpec &fs, Slot slot, double *grad_dst, unsigned index, double *value);
     bool eval_user_objective(Slot slot, bool want_grad, double *value);
+    bool negate_gradient(double *g);
     bool push_rows_to(double *dst, unsigned rows, const double *host_grad);
     bool eval_penalty_objective(Slot slot, bool want_grad, double *value);
     bool dual_eval(const double *y, const DualScalars &sc, bool materialize, DualSums *out) override;

@@ -322,29 +322,40 @@ nlopt_result nlopt_set_max_objective(nlopt_opt opt, nlopt_func f, void *d)
 { return set_objective(opt, f, nullptr, nullptr, d, 1); }
 nlopt_result nlopt_b200_set_min_objective_device(nlopt_opt opt, nlopt_b200_dfunc f, void *d)
 { return set_objective(opt, nullptr, f, nullptr, d, 0); }
+nlopt_result nlopt_b200_set_max_objective_device(nlopt_opt opt, nlopt_b200_dfunc f, void *d)
+{ return set_objective(opt, nullptr, f, nullptr, d, 1); }
 
 /* marker stored in the `df` field of callbacks registered in the asynchronous form: never called */
 static double df2_marker(unsigned, unsigned long long, const double *, double *, void *, void *) { return 0.0; }
 
-nlopt_result nlopt_b200_set_min_objective_device2(nlopt_opt opt, nlopt_b200_dfunc2 f, nlopt_b200_dfinish fin, void *d, int halo)
+static nlopt_result set_objective_device2(nlopt_opt opt, nlopt_b200_dfunc2 f, nlopt_b200_dfinish fin, void *d, int halo,
+                                          int maximize)
 {
     if (!f || !fin || halo < 0 || halo > 1) return NLOPT_INVALID_ARGS;
-    nlopt_result r = set_objective(opt, nullptr, df2_marker, nullptr, d, 0);
+    nlopt_result r = set_objective(opt, nullptr, df2_marker, nullptr, d, maximize);
     if (r < 0) return r;
     opt->df2 = f;
     opt->dfin = fin;
     opt->halo = halo;
     return r;
 }
+nlopt_result nlopt_b200_set_min_objective_device2(nlopt_opt opt, nlopt_b200_dfunc2 f, nlopt_b200_dfinish fin, void *d, int halo)
+{ return set_objective_device2(opt, f, fin, d, halo, 0); }
+nlopt_result nlopt_b200_set_max_objective_device2(nlopt_opt opt, nlopt_b200_dfunc2 f, nlopt_b200_dfinish fin, void *d, int halo)
+{ return set_objective_device2(opt, f, fin, d, halo, 1); }
 
-nlopt_result nlopt_b200_set_min_objective_sharded(nlopt_opt opt, nlopt_b200_sfunc f, void *d)
+static nlopt_result set_objective_sharded(nlopt_opt opt, nlopt_b200_sfunc f, void *d, int maximize)
 {
     if (!f) return NLOPT_INVALID_ARGS;
-    nlopt_result r = set_objective(opt, nullptr, df2_marker, nullptr, d, 0);
+    nlopt_result r = set_objective(opt, nullptr, df2_marker, nullptr, d, maximize);
     if (r < 0) return r;
     opt->sf = f;
     return r;
 }
+nlopt_result nlopt_b200_set_min_objective_sharded(nlopt_opt opt, nlopt_b200_sfunc f, void *d)
+{ return set_objective_sharded(opt, f, d, 0); }
+nlopt_result nlopt_b200_set_max_objective_sharded(nlopt_opt opt, nlopt_b200_sfunc f, void *d)
+{ return set_objective_sharded(opt, f, d, 1); }
 
 nlopt_algorithm nlopt_get_algorithm(const nlopt_opt opt) { return opt->algorithm; }
 unsigned nlopt_get_dimension(const nlopt_opt opt) { return opt->n; }
@@ -790,15 +801,19 @@ static nlopt_result optimize_common(nlopt_opt opt, double *x_host, double *x_dev
     nlopt_set_force_stop(opt, 0);
     opt->force_stop_child = nullptr;
 
-    /* maximisation: minimise the sign-flipped objective, then restore (optimize.c:1014-1024, :1070-1077) */
+    /* maximisation: minimise the sign-flipped objective, then restore (optimize.c:1014-1024, :1070-1077).  A host
+       objective is wrapped in flipped(); a device or sharded objective keeps its callback and the backend negates its
+       final value and its gradient (opt->negate -> FuncSpec::negate) */
     nlopt_func f0 = opt->f;
     void *d0 = opt->f_data;
     FlipData flip{f0, d0};
     const int maximize = opt->maximize;
     if (maximize) {
-        if (!opt->f) { set_err(opt, "maximisation needs a host objective"); return NLOPT_INVALID_ARGS; }
-        opt->f = flipped;
-        opt->f_data = &flip;
+        if (opt->f) {
+            opt->f = flipped;
+            opt->f_data = &flip;
+        } else
+            opt->negate = 1;
         opt->stopval = -opt->stopval;
         opt->maximize = 0;
     }
@@ -809,6 +824,7 @@ static nlopt_result optimize_common(nlopt_opt opt, double *x_host, double *x_dev
         ret = run_ccsa(opt, x_host, x_dev, opt_f);
     if (maximize) {
         opt->maximize = maximize;
+        opt->negate = 0;
         opt->stopval = -opt->stopval;
         opt->f = f0;
         opt->f_data = d0;
@@ -984,6 +1000,7 @@ nlopt_result run_ccsa(nlopt_opt opt, double *x_host, double *x_dev, double *minf
     cfg.objective.halo = opt->halo;
     cfg.objective.sf = opt->sf;
     cfg.objective.data = opt->f_data;
+    cfg.objective.negate = opt->negate != 0;
     cfg.penalty = opt->penalty;
     std::vector<double> tol;
     for (const auto &c : opt->fc) {
@@ -1408,6 +1425,7 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
         ~Cleanup()
         {
             sub->penalty = nullptr;
+            sub->negate = 0;
             opt->force_stop_child = nullptr;
             if (own) nlopt_destroy(sub);
         }
@@ -1454,6 +1472,7 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
     sub->halo = opt->halo;
     sub->pre = nullptr;
     sub->maximize = 0;
+    sub->negate = opt->negate;          /* a maximised device objective: the sub-problem's L starts from -f */
     nlopt_set_lower_bounds(sub, opt->lb.data());
     nlopt_set_upper_bounds(sub, opt->ub.data());
     sub->lb_uniform = opt->lb_uniform;
@@ -1487,7 +1506,7 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
         vc.values_only = true;
         vc.n = n;
         vc.objective.f = opt->f; vc.objective.df = opt->df; vc.objective.df2 = opt->df2; vc.objective.dfin = opt->dfin;
-        vc.objective.halo = opt->halo; vc.objective.data = opt->f_data;
+        vc.objective.halo = opt->halo; vc.objective.data = opt->f_data; vc.objective.negate = opt->negate != 0;
         for (const auto &c : opt->h) vc.constraints.push_back(to_spec(c));
         for (const auto &c : pen_fc) vc.constraints.push_back(to_spec(c));
         vc.lb = opt->lb.data();

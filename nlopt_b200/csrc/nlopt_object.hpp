@@ -49,6 +49,7 @@ struct nlopt_opt_s {
     void *f_data = nullptr;
     nlopt_precond pre = nullptr;
     int maximize = 0;
+    int negate = 0;         // while a maximisation with a device or sharded objective runs: the backend negates f
 
     std::vector<nb200::NamedParam *> params;      // pointers stay valid: nlopt_nth_param hands out c_str()
 

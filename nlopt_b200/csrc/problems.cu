@@ -121,6 +121,30 @@ struct SphereDev {
     double finish(double s) const { return s * inv_n - r; }
 };
 
+// -F, for maximisation: term -F(...), gradient -grad F, finish(s) = -F.finish(-s).  Negation is exact and a sum of
+// negated terms in the same tree is the negated sum, so the library's minimisation of -(-F) -- value and gradient
+// negated once more -- sees F's bits: a max run of Negated<F> is the min run of F.
+template <class F>
+struct Negated {
+    static constexpr int halo = nlopt_b200::detail::halo_of<F>::value;
+    F f;
+    __device__ double operator()(unsigned long long j, unsigned long long n, long long jl, long long n_local,
+                                 const double *x, double *grad_j) const
+    {
+        const double t = f(j, n, jl, n_local, x, grad_j);
+        if (grad_j) *grad_j = -*grad_j;
+        return -t;
+    }
+    double finish(double s) const { return -f.finish(-s); }
+};
+
+template <class F>
+int set_objective(nlopt_opt opt, const F *f, int sync, int maximize)
+{
+    if (maximize) return sync ? nlopt_b200::set_max_objective_sync(opt, f) : nlopt_b200::set_max_objective(opt, f);
+    return sync ? nlopt_b200::set_min_objective_sync(opt, f) : nlopt_b200::set_min_objective(opt, f);
+}
+
 template <class F>
 int add_eq(nlopt_opt opt, const F *f, double tol, int sync)
 {
@@ -223,6 +247,9 @@ struct nb200p_problem_s {
     std::vector<double *> dev_rows;
     std::vector<nb200p_lin_data *> lin_host;
     SimpDev simp;
+    Negated<RosenbrockDev> nrosen;          // maximisation twins (nb200p_set_*_device_max)
+    Negated<QuadraticDev> nquad;
+    Negated<SimpDev> nsimp;
     std::vector<void *> misc_host;          // small data records of the host callbacks (freed with the problem)
     std::vector<std::shared_ptr<void>> vec; // vector functors (LinearRowsDev<M>, BlockMeanDev<M>)
 };
@@ -392,6 +419,57 @@ int nb200p_set_simp_device(nb200p_problem_s *p, nlopt_opt opt, unsigned long lon
     return nlopt_b200::set_min_objective(opt, &p->simp);
 }
 
+// ---- maximisation: Negated<F> through nlopt_b200::set_max_objective (sync != 0: set_max_objective_sync) ----------------
+int nb200p_set_quadratic_device_max(nb200p_problem_s *p, nlopt_opt opt, unsigned long long seed, int sync)
+{
+    p->nquad.f.seed = seed;
+    return set_objective(opt, &p->nquad, sync, 1);
+}
+
+int nb200p_set_simp_device_max(nb200p_problem_s *p, nlopt_opt opt, unsigned long long seed, double eps, int sync)
+{
+    p->nsimp.f.seed = seed;
+    p->nsimp.f.eps = eps;
+    return set_objective(opt, &p->nsimp, sync, 1);
+}
+
+// the chained Rosenbrock function (halo 1), minimised or, as Negated<RosenbrockDev>, maximised, in either form
+int nb200p_set_rosenbrock_device_form(nb200p_problem_s *p, nlopt_opt opt, int sync, int maximize)
+{
+    return maximize ? set_objective(opt, &p->nrosen, sync, 1) : set_objective(opt, &p->rosen, sync, 0);
+}
+
+// The raw pointers the C++ front end registers for QuadraticDev (negated != 0: Negated<QuadraticDev>), for registration
+// from another language: sync == 0: nlopt_b200_dfunc2 / nlopt_b200_dfinish and the functor; sync != 0: nlopt_b200_dfunc
+// and its data record (*fin = NULL)
+int nb200p_quadratic_pointers(nb200p_problem_s *p, nlopt_opt opt, unsigned long long seed, int negated, int sync, void **fn,
+                              void **fin, void **data)
+{
+    namespace d = nlopt_b200::detail;
+    p->quad.seed = seed;
+    p->nquad.f.seed = seed;
+    const unsigned long long n = nlopt_get_dimension(opt);
+    if (sync) {
+        *fin = nullptr;
+        if (negated) {
+            *fn = (void *) &d::trampoline<Negated<QuadraticDev>>;
+            *data = new d::Bound<Negated<QuadraticDev>>{&p->nquad, n};     // lives as long as the process, as in the front end
+        } else {
+            *fn = (void *) &d::trampoline<QuadraticDev>;
+            *data = new d::Bound<QuadraticDev>{&p->quad, n};
+        }
+    } else if (negated) {
+        *fn = (void *) &d::trampoline2<Negated<QuadraticDev>>;
+        *fin = (void *) &d::finish2<Negated<QuadraticDev>>;
+        *data = &p->nquad;
+    } else {
+        *fn = (void *) &d::trampoline2<QuadraticDev>;
+        *fin = (void *) &d::finish2<QuadraticDev>;
+        *data = &p->quad;
+    }
+    return NLOPT_SUCCESS;
+}
+
 // ---- host callbacks (nlopt_func shape; work with any NLopt-ABI library) ----------------------------------
 double nb200p_simp_host(unsigned n, const double *x, double *grad, void *data)
 {
@@ -424,6 +502,16 @@ double nb200p_simp_sharded(unsigned n_local, unsigned long long j0, unsigned lon
         f += a / d;
     }
     return f;
+}
+
+// -nb200p_simp_sharded, value and gradient (nlopt_b200_set_max_objective_sharded)
+double nb200p_simp_sharded_neg(unsigned n_local, unsigned long long j0, unsigned long long n, const double *x, double *grad,
+                               void *data)
+{
+    const double f = nb200p_simp_sharded(n_local, j0, n, x, grad, data);
+    if (grad)
+        for (unsigned jl = 0; jl < n_local; ++jl) grad[jl] = -grad[jl];
+    return -f;
 }
 
 double nb200p_mean_sharded(unsigned n_local, unsigned long long j0, unsigned long long n, const double *x, double *grad, void *data)

@@ -34,6 +34,11 @@ def _load():
     L.nb200p_add_mean_device_sync.argtypes = [C.c_void_p, C.c_void_p, C.c_double, C.c_double]
     L.nb200p_add_linear_rows_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint, c_double_p, c_double_p, c_double_p, C.c_int]
     L.nb200p_add_block_mean_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint, c_double_p, c_double_p, C.c_int]
+    L.nb200p_set_quadratic_device_max.argtypes = [C.c_void_p, C.c_void_p, C.c_ulonglong, C.c_int]
+    L.nb200p_set_simp_device_max.argtypes = [C.c_void_p, C.c_void_p, C.c_ulonglong, C.c_double, C.c_int]
+    L.nb200p_set_rosenbrock_device_form.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
+    L.nb200p_quadratic_pointers.argtypes = [C.c_void_p, C.c_void_p, C.c_ulonglong, C.c_int, C.c_int,
+                                            C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
     for nm, args in (("nb200p_make_simp_data", [C.c_void_p, C.c_ulonglong, C.c_double]),
                      ("nb200p_make_mean_data", [C.c_void_p, C.c_double]), ("nb200p_make_quad_data", [C.c_void_p, C.c_ulonglong])):
         getattr(L, nm).restype = C.c_void_p
@@ -126,6 +131,36 @@ class Problem:
     def set_simp_device(self, opt, seed=0x5EED0000, eps=1e-3, sync=False):
         fn = self.L.nb200p_set_simp_device_sync if sync else self.L.nb200p_set_simp_device
         opt._check(fn(self.h, opt._h, seed, eps))
+
+    # ---- maximisation: the negated functors (Negated<F> in problems.cu) through set_max_objective ----
+    # A max run of the negated functor is the min run of the functor itself, bit for bit.
+    def set_quadratic_device_max(self, opt, seed=0x5EED0000, sync=False):
+        """maximise -(config 2 quadratic)"""
+        opt._check(self.L.nb200p_set_quadratic_device_max(self.h, opt._h, seed, int(sync)))
+
+    def set_simp_device_max(self, opt, seed=0x5EED0000, eps=1e-3, sync=False):
+        """maximise -(SIMP compliance)"""
+        opt._check(self.L.nb200p_set_simp_device_max(self.h, opt._h, seed, eps, int(sync)))
+
+    def set_rosenbrock_device(self, opt, sync=False, maximize=False):
+        """the chained Rosenbrock objective alone (halo 1); maximize=True registers its negation with set_max_objective"""
+        opt._check(self.L.nb200p_set_rosenbrock_device_form(self.h, opt._h, int(sync), int(maximize)))
+
+    def quadratic_pointers(self, opt, seed=0x5EED0000, negated=False, sync=False):
+        """(fn, finish, data) pointers of the quadratic functor, or of its negation, as the C++ front end registers them:
+        nlopt_b200_dfunc2 / nlopt_b200_dfinish, or with sync=True an nlopt_b200_dfunc (finish None)"""
+        fn, fin, data = C.c_void_p(), C.c_void_p(), C.c_void_p()
+        opt._check(self.L.nb200p_quadratic_pointers(self.h, opt._h, seed, int(negated), int(sync), C.byref(fn), C.byref(fin),
+                                                    C.byref(data)))
+        return fn, fin, data
+
+    def simp_sharded_max(self, opt, seed=0x5EED0000, eps=1e-3, vol=0.4, tol=0.0):
+        """simp_sharded with the negated objective registered by nlopt_b200_set_max_objective_sharded"""
+        lib_ = opt._lib
+        d = self.L.nb200p_make_simp_data(self.h, seed, eps)
+        opt._check(lib_.nlopt_b200_set_max_objective_sharded(opt._h, C.cast(self.L.nb200p_simp_sharded_neg, C.c_void_p), d))
+        dm = self.L.nb200p_make_mean_data(self.h, -vol)
+        opt._check(lib_.nlopt_b200_add_inequality_constraint_sharded(opt._h, C.cast(self.L.nb200p_mean_sharded, C.c_void_p), dm, tol))
 
     def add_mean_device(self, opt, offset, tol=0.0, sync=False):
         """inequality  mean(x) + offset <= 0"""
