@@ -287,6 +287,36 @@ nlopt_result nlopt_b200_add_inequality_mconstraint_device2(nlopt_opt opt, unsign
 nlopt_result nlopt_b200_add_equality_mconstraint_device2(nlopt_opt opt, unsigned m, nlopt_b200_dmfunc2 h,
                                                          nlopt_b200_dmfinish finish, void *h_data, const double *tol,
                                                          int halo);
+/* Device callbacks, third form: per-variable TERMS, for code that cannot be written as a __device__ functor (its own
+ * kernels, cuBLAS / cuSPARSE, a filter, PyTorch).  The callback enqueues on `cuda_stream`, and does not synchronise:
+ *     terms_dev[i * ld + jl] = term i of variable j0 + jl          (i < m, jl < shard->n_local)
+ * and, when grad_dev != NULL, grad_dev[i * ld + jl] = d c_i / d x_j (m = 1 for a scalar function).  terms_dev is a
+ * library-owned buffer of m * ld doubles (ld >= n_local; entries from n_local to ld are never read); it is valid only
+ * for the duration of the call and the work the callback enqueues.  The library then reduces row i of the terms on the
+ * GPU in exactly the order of the __device__ functors (nlopt_b200_device.cuh: map_group_kernel / map_group_mkernel
+ * and the fold of the group sums), adds the 8 virtual-shard sums in index order and calls finish once per point, as
+ * for the _device2 forms: finish(total, data) for a scalar function, finish(m, totals, result, data) for m rows.
+ * Bit contract: terms bit-equal to a functor's terms give that functor's value bits, so a run matches the functor's run
+ * bit for bit (result code, evaluation counts, f*, x*) under LD_MMA, LD_CCSAQ and the AUGLAG family; the value depends
+ * on n only, not on the number of ranks.  `halo` as for the _device2 forms (the callback may read x_dev[-1] and
+ * x_dev[n_local]).  Argument checks are those of the _device2 / _mconstraint_device2 twins; any m the constraint path
+ * accepts (no register-file cap).  Not taken by preconditioned CCSAQ. */
+typedef void (*nlopt_b200_dtfunc)(unsigned m, const nlopt_b200_shard *shard, const double *x_dev, double *grad_dev,
+                                  unsigned long long ld, double *terms_dev, void *func_data, void *cuda_stream);
+nlopt_result nlopt_b200_set_min_objective_terms(nlopt_opt opt, nlopt_b200_dtfunc f, nlopt_b200_dfinish finish,
+                                                void *f_data, int halo);
+nlopt_result nlopt_b200_set_max_objective_terms(nlopt_opt opt, nlopt_b200_dtfunc f, nlopt_b200_dfinish finish,
+                                                void *f_data, int halo);
+nlopt_result nlopt_b200_add_inequality_constraint_terms(nlopt_opt opt, nlopt_b200_dtfunc fc, nlopt_b200_dfinish finish,
+                                                        void *fc_data, double tol, int halo);
+nlopt_result nlopt_b200_add_equality_constraint_terms(nlopt_opt opt, nlopt_b200_dtfunc h, nlopt_b200_dfinish finish,
+                                                      void *h_data, double tol, int halo);
+nlopt_result nlopt_b200_add_inequality_mconstraint_terms(nlopt_opt opt, unsigned m, nlopt_b200_dtfunc fc,
+                                                         nlopt_b200_dmfinish finish, void *fc_data, const double *tol,
+                                                         int halo);
+nlopt_result nlopt_b200_add_equality_mconstraint_terms(nlopt_opt opt, unsigned m, nlopt_b200_dtfunc h,
+                                                       nlopt_b200_dmfinish finish, void *h_data, const double *tol,
+                                                       int halo);
 /* Sharded HOST callbacks (one process per GPU): the callback sees only this rank's variables -- x_shard and grad_shard
  * hold the n_local entries starting at global index j0 -- and returns its ADDITIVE contribution to the function value
  * (a constant term is added by one rank only, e.g. the one with j0 == 0); the library sums the contributions over the

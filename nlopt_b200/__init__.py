@@ -17,8 +17,8 @@ import ctypes as C
 
 import numpy as np
 
-from ._capi import (NLOPT_B200_DFUNC, NLOPT_FUNC, NLOPT_PRECOND, NLOPT_MFUNC, Library, Stats, c_double_p,
-                    default_library)
+from ._capi import (NLOPT_B200_DFINISH, NLOPT_B200_DFUNC, NLOPT_B200_DMFINISH, NLOPT_B200_DTFUNC, NLOPT_FUNC,
+                    NLOPT_PRECOND, NLOPT_MFUNC, Library, Shard, Stats, c_double_p, default_library)
 
 # --- algorithm ids (reference nlopt.h:72-154) ---------------------------------
 _ALG_NAMES = [
@@ -59,6 +59,15 @@ def _ptr(a):
     return a.ctypes.data_as(c_double_p)
 
 
+class _DeviceArray:
+    """float64 device memory of the library, handed to torch.as_tensor as a zero-copy view (no stream: the view is
+    used on the library stream itself)"""
+
+    def __init__(self, ptr, shape, strides):
+        self.__cuda_array_interface__ = {"shape": shape, "strides": strides, "typestr": "<f8", "data": (ptr, False),
+                                         "version": 2}
+
+
 class opt:
     """One optimisation problem; thin owner of an ``nlopt_opt`` handle."""
 
@@ -70,6 +79,7 @@ class opt:
         self._n = int(n)
         self._keep = []            # ctypes thunks must outlive the handle
         self._exc = None           # exception raised inside a callback
+        self._tviews = {}          # torch callbacks: zero-copy views and external streams, per pointer (one run)
         self._last_result = FAILURE
         self._last_optf = float("inf")
 
@@ -210,6 +220,128 @@ class opt:
         tol = _as_f64(tol)
         self._check(self._lib.nlopt_b200_add_equality_mconstraint_device2(
             self._h, tol.size, fn_ptr, finish_ptr, data_ptr, _ptr(tol), int(halo)))
+
+    # ---- extension: PyTorch callbacks (per-variable terms, nlopt_b200_dtfunc) ---------------------------------------
+    # f(x, grad) gets zero-copy float64 CUDA views of the library's HBM: x (n_local entries; with halo=1 n_local + 2,
+    # x[0] being the left neighbour x[-1]) and grad, written in place -- (n_local,), or (m, n_local) with row stride ld
+    # for the vector form; empty (numel() == 0) when no gradient is wanted.  f returns the terms, whose sum is the
+    # function: a float64 tensor of grad's shape.  The library reduces them on the GPU in the order of the __device__
+    # functors and applies finish once per point (default: the identity; vector form: m totals -> m values, numpy).
+    # f runs on the library's stream (torch.cuda.ExternalStream), so its kernels are ordered with the library's.
+    def _tcached(self, key, make):
+        v = self._tviews.get(key)
+        if v is None:
+            v = self._tviews[key] = make()
+        return v
+
+    def _wrap_terms(self, f, vector, halo):
+        import torch
+
+        def view(ptr, shape, strides):
+            return self._tcached((ptr, shape, strides), lambda: torch.as_tensor(_DeviceArray(ptr, shape, strides)))
+
+        def thunk(m, shard, x, grad, ld, terms, _data, stream):
+            try:
+                nl_ = Shard.from_address(shard).n_local
+                shape, strides = ((m, nl_), (8 * ld, 8)) if vector else ((nl_,), (8,))
+                xv = view(x - 8 * halo, (nl_ + 2 * halo,), (8,))
+                tv = view(terms, shape, strides)
+                gv = view(grad, shape, strides) if grad else self._tcached(
+                    ("empty", xv.device), lambda: torch.empty(0, dtype=torch.float64, device=xv.device))
+                s = self._tcached(("stream", stream), lambda: torch.cuda.ExternalStream(stream, device=xv.device))
+                with torch.cuda.stream(s):
+                    out = f(xv, gv)
+                    if not (isinstance(out, torch.Tensor) and out.dtype == torch.float64 and out.device == tv.device
+                            and tuple(out.shape) == shape):
+                        raise ValueError(f"a torch terms callback returns a float64 tensor of shape {shape} on {tv.device}")
+                    tv.copy_(out)
+            except BaseException as e:
+                self._exc = e
+                self._lib.nlopt_force_stop(self._h)
+
+        cb = NLOPT_B200_DTFUNC(thunk)
+        self._keep.append(cb)
+        return C.cast(cb, C.c_void_p)
+
+    def _wrap_finish(self, finish):
+        def thunk(total, _data):
+            try:
+                return float(total if finish is None else finish(total))
+            except BaseException as e:
+                self._exc = e
+                self._lib.nlopt_force_stop(self._h)
+                return float("nan")
+
+        cb = NLOPT_B200_DFINISH(thunk)
+        self._keep.append(cb)
+        return C.cast(cb, C.c_void_p)
+
+    def _wrap_mfinish(self, finish):
+        def thunk(m, totals, result, _data):
+            try:
+                t = np.ctypeslib.as_array(totals, shape=(m,)).copy()
+                np.ctypeslib.as_array(result, shape=(m,))[:] = t if finish is None else finish(t)
+            except BaseException as e:
+                self._exc = e
+                self._lib.nlopt_force_stop(self._h)
+
+        cb = NLOPT_B200_DMFINISH(thunk)
+        self._keep.append(cb)
+        return C.cast(cb, C.c_void_p)
+
+    def set_min_objective_torch(self, f, finish=None, halo=0):
+        self._check(self._lib.nlopt_b200_set_min_objective_terms(
+            self._h, self._wrap_terms(f, False, halo), self._wrap_finish(finish), None, int(halo)))
+
+    def set_max_objective_torch(self, f, finish=None, halo=0):
+        self._check(self._lib.nlopt_b200_set_max_objective_terms(
+            self._h, self._wrap_terms(f, False, halo), self._wrap_finish(finish), None, int(halo)))
+
+    def add_inequality_constraint_torch(self, fc, tol=0.0, finish=None, halo=0):
+        self._check(self._lib.nlopt_b200_add_inequality_constraint_terms(
+            self._h, self._wrap_terms(fc, False, halo), self._wrap_finish(finish), None, float(tol), int(halo)))
+
+    def add_equality_constraint_torch(self, h, tol=0.0, finish=None, halo=0):
+        self._check(self._lib.nlopt_b200_add_equality_constraint_terms(
+            self._h, self._wrap_terms(h, False, halo), self._wrap_finish(finish), None, float(tol), int(halo)))
+
+    # m = len(tol) rows: f returns (m, n_local) terms
+    def add_inequality_mconstraint_torch(self, fc, tol, finish=None, halo=0):
+        tol = _as_f64(tol)
+        self._check(self._lib.nlopt_b200_add_inequality_mconstraint_terms(
+            self._h, tol.size, self._wrap_terms(fc, True, halo), self._wrap_mfinish(finish), None, _ptr(tol), int(halo)))
+
+    def add_equality_mconstraint_torch(self, h, tol, finish=None, halo=0):
+        tol = _as_f64(tol)
+        self._check(self._lib.nlopt_b200_add_equality_mconstraint_terms(
+            self._h, tol.size, self._wrap_terms(h, True, halo), self._wrap_mfinish(finish), None, _ptr(tol), int(halo)))
+
+    def optimize_torch(self, x):
+        """nlopt_b200_optimize_device on a torch tensor: x (contiguous float64 CUDA tensor of this rank's n_local
+        variables) holds the start point on entry and the solution on return; last_optimum_value() is the optimum.
+        Torch's current stream is synchronised first, so x is ready.  Returns x."""
+        import torch
+        j0, cnt = C.c_ulonglong(), C.c_ulonglong()
+        lib = self._lib
+        lib.nlopt_b200_shard_range(self._n, lib.nlopt_b200_comm_rank(), lib.nlopt_b200_comm_world(), C.byref(j0), C.byref(cnt))
+        if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dtype == torch.float64 and x.is_contiguous()
+                and x.numel() == cnt.value):
+            raise ValueError(f"optimize_torch needs a contiguous float64 CUDA tensor of this rank's {cnt.value} variables")
+        f = C.c_double(0.0)
+        self._exc = None
+        self._tviews.clear()
+        with torch.cuda.device(x.device):
+            torch.cuda.current_stream().synchronize()
+            try:
+                ret = lib.nlopt_b200_optimize_device(self._h, x.data_ptr(), C.byref(f))
+            finally:
+                self._tviews.clear()
+        self._last_result, self._last_optf = ret, f.value
+        if ret == FORCED_STOP and self._exc is not None:
+            e, self._exc = self._exc, None
+            raise e
+        self._check(ret)
+        return x
 
     def optimize_device(self, x_dev_ptr):
         f = C.c_double(0.0)

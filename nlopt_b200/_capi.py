@@ -19,6 +19,19 @@ NLOPT_PRECOND = C.CFUNCTYPE(None, C.c_uint, c_double_p, c_double_p, c_double_p, 
 # extension: device callback (include/nlopt_b200.h)
 NLOPT_B200_DFUNC = C.CFUNCTYPE(C.c_double, C.c_uint, C.c_ulonglong, C.c_void_p, C.c_void_p,
                                C.c_void_p, C.c_void_p)
+# terms callbacks (nlopt_b200_dtfunc) and the host finishes of the asynchronous forms
+NLOPT_B200_DTFUNC = C.CFUNCTYPE(None, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p, C.c_ulonglong, C.c_void_p,
+                                C.c_void_p, C.c_void_p)
+NLOPT_B200_DFINISH = C.CFUNCTYPE(C.c_double, C.c_double, C.c_void_p)
+NLOPT_B200_DMFINISH = C.CFUNCTYPE(None, C.c_uint, c_double_p, c_double_p, C.c_void_p)
+
+
+class Shard(C.Structure):
+    """nlopt_b200_shard: this rank's part of the library's variable / group / virtual-shard geometry"""
+    _fields_ = [("n", C.c_ulonglong), ("n_local", C.c_ulonglong), ("j0", C.c_ulonglong), ("nchunks", C.c_ulonglong),
+                ("chunk0", C.c_ulonglong), ("groups_total", C.c_uint), ("group0", C.c_uint), ("groups_local", C.c_uint),
+                ("groups_per_vshard", C.c_uint), ("vshard0", C.c_uint), ("local_vshards", C.c_uint), ("rank", C.c_int),
+                ("world", C.c_int)]
 
 PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 REPO_DIR = os.path.dirname(PKG_DIR)
@@ -151,6 +164,16 @@ _EXT = {
     "nlopt_b200_add_inequality_mconstraint_device2":
         (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p, c_double_p, C.c_int]),
     "nlopt_b200_add_equality_mconstraint_device2":
+        (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p, c_double_p, C.c_int]),
+    "nlopt_b200_set_min_objective_terms": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
+    "nlopt_b200_set_max_objective_terms": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
+    "nlopt_b200_add_inequality_constraint_terms":
+        (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_int]),
+    "nlopt_b200_add_equality_constraint_terms":
+        (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_int]),
+    "nlopt_b200_add_inequality_mconstraint_terms":
+        (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p, c_double_p, C.c_int]),
+    "nlopt_b200_add_equality_mconstraint_terms":
         (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p, c_double_p, C.c_int]),
     "nlopt_b200_shard_geometry": (None, [C.c_ulonglong, C.c_int, C.c_int, C.c_void_p]),
     "nlopt_b200_set_min_objective_sharded": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -22,11 +22,16 @@ struct FuncSpec {
     nlopt_b200_dfinish dfin = nullptr;       // ... and its host-side finish
     nlopt_b200_dmfunc2 dmf2 = nullptr;       // vector asynchronous device callback, m rows (constraints only) ...
     nlopt_b200_dmfinish dmfin = nullptr;     // ... and its host-side finish of the m totals
+    nlopt_b200_dtfunc dtf = nullptr;         // per-variable terms, m rows, reduced by the library; finish in dfin, or in
+                                             // dmfin for the vector form
     int halo = 0;
     nlopt_b200_sfunc sf = nullptr;           // sharded host callback
     void *data = nullptr;
     bool negate = false;                     // objective of a maximisation (device / sharded callbacks only): the
                                              // backend minimises -f -- final value and gradient change sign
+
+    // an asynchronous device callback: enqueued on the library stream, its value settled by finish_evals()
+    bool async_device() const { return df2 || dmf2 || dtf; }
 };
 
 // The augmented-Lagrangian objective of NLOPT_AUGLAG* (src/algs/auglag/auglag.c:25-65), evaluated by the backend:

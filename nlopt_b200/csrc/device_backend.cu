@@ -16,6 +16,7 @@
 #include "comm.hpp"
 #include "dual_mma.hpp"
 #include "synth.cuh"
+#include "terms_kernels.cuh"
 
 namespace nb200 {
 
@@ -220,6 +221,7 @@ void DeviceBackend::free_state()
     if (xfull_dev_) BlockCache::get().give(false, (size_t) Comm::instance().world * shard_cap_ * sizeof(double), xfull_dev_, device_);
     solve_state_ = nullptr;
     vs2_dev_ = vs2_host_ = halo_edges_ = nullptr;
+    terms_ = terms_part_ = nullptr;
     halo_ptr_ = nullptr;
     grouptags_ = nullptr;
     res_host_ = nullptr;
@@ -400,6 +402,16 @@ bool DeviceBackend::setup(const BackendConfig &cfg)
                 pen_total_ += c.m;
                 if (c.m > max_cdim_) max_cdim_ = c.m;
             }
+    terms_rows_ = cfg.objective.dtf ? 1 : 0;
+    auto terms_rows_of = [this](const std::vector<FuncSpec> &list) {
+        for (const FuncSpec &c : list)
+            if (c.dtf && c.m > terms_rows_) terms_rows_ = c.m;
+    };
+    terms_rows_of(cfg.constraints);
+    if (cfg.penalty) {
+        terms_rows_of(cfg.penalty->eq);
+        terms_rows_of(cfg.penalty->ineq);
+    }
     if (cfg.stats) stats_ = cfg.stats;
     if (!alloc_state()) return false;
     const size_t nl = geo_.n_local, j0 = geo_.j0;
@@ -653,7 +665,7 @@ bool DeviceBackend::eval_penalty_objective(Slot slot, bool want_grad, double *va
         unsigned row = 0;
         for (int pass = 0; pass < 2; ++pass)
             for (const FuncSpec &fs : (pass == 0 ? ps.eq : ps.ineq)) {
-                if ((fs.df2 || fs.dmf2) && !enqueue_df2(fs, slot, want_grad ? pen_rows_ + (size_t) row * geo_.ld : nullptr, 1 + m_ + row))
+                if (fs.async_device() && !enqueue_df2(fs, slot, want_grad ? pen_rows_ + (size_t) row * geo_.ld : nullptr, 1 + m_ + row))
                     return false;
                 row += fs.m;
             }
@@ -670,7 +682,7 @@ bool DeviceBackend::eval_penalty_objective(Slot slot, bool want_grad, double *va
     bool any_partial = false;
     for (int pass = 0; pass < 2; ++pass)
         for (const FuncSpec &fs : (pass == 0 ? ps.eq : ps.ineq)) {
-            if (fs.df2 || fs.dmf2) {
+            if (fs.async_device()) {
                 for (unsigned r = 0; r < fs.m; ++r) vals[row + r] = settled[m_ + row + r];
             } else if (fs.df) {
                 const double t0 = wall_seconds();
@@ -773,7 +785,7 @@ bool DeviceBackend::eval_user_objective(Slot slot, bool want_grad, double *value
         if (fs.negate && !Comm::instance().active()) *value = -*value;
         return !fs.negate || negate_gradient(gs);
     }
-    if (fs.df2) {
+    if (fs.async_device()) {
         double *gs = want_grad ? (slot == kBase ? g_ : gcur_) : nullptr;
         *value = 0.0;                                  // settled in finish_evals()
         if (!enqueue_df2(fs, slot, gs, 0)) return false;
@@ -808,7 +820,7 @@ bool DeviceBackend::eval_constraint(Slot slot, unsigned ic, unsigned row0, bool 
 {
     const FuncSpec &fs = cfg_.constraints[ic];
     if (fs.sf) return eval_sharded(fs, slot, want_grad ? (slot == kBase ? G_ : Gcur_) + (size_t) row0 * geo_.ld : nullptr, 1 + row0, values);
-    if (fs.df2 || fs.dmf2) {
+    if (fs.async_device()) {
         double *gs = want_grad ? (slot == kBase ? G_ : Gcur_) + (size_t) row0 * geo_.ld : nullptr;
         for (unsigned r = 0; r < fs.m; ++r) values[r] = 0.0;
         return enqueue_df2(fs, slot, gs, 1 + row0);
@@ -879,7 +891,8 @@ bool DeviceBackend::eval_sharded(const FuncSpec &fs, Slot slot, double *grad_dst
 }
 
 // Asynchronous device callbacks (nlopt_b200_dfunc2): enqueue, remember which value is pending.  A vector callback
-// (nlopt_b200_dmfunc2) takes the m slots [index, index + m) and the m gradient rows from grad_dst on, stride ld.
+// (nlopt_b200_dmfunc2) takes the m slots [index, index + m) and the m gradient rows from grad_dst on, stride ld; so does
+// a terms callback (nlopt_b200_dtfunc, reduce_terms) of m rows.
 bool DeviceBackend::enqueue_df2(const FuncSpec &fs, Slot slot, double *grad_dst, unsigned index)
 {
     Comm &comm = Comm::instance();
@@ -897,13 +910,43 @@ bool DeviceBackend::enqueue_df2(const FuncSpec &fs, Slot slot, double *grad_dst,
     if (!pend2_any_) NB_CUDA(cudaMemsetAsync(vs2_dev_, 0, vs2_cap_ * kV * sizeof(double), stream_));   // first callback of this point
     if (fs.halo > 0 && !ensure_halo(slot)) return false;
     double *xs = slot == kBase ? x_ : xcur_view();
-    const double t0 = wall_seconds();
-    if (fs.dmf2) fs.dmf2(fs.m, &shard_, xs, grad_dst, geo_.ld, vs2_dev_ + (size_t) index * kV, fs.data, stream_);
-    else fs.df2(&shard_, xs, grad_dst, vs2_dev_ + (size_t) index * kV, fs.data, stream_);
-    cb_seconds_ += wall_seconds() - t0;
-    NB_CUDA(cudaGetLastError());
+    double *vsums = vs2_dev_ + (size_t) index * kV;
+    if (fs.dtf) {
+        if (!reduce_terms(fs, xs, grad_dst, vsums)) return false;
+    } else {
+        const double t0 = wall_seconds();
+        if (fs.dmf2) fs.dmf2(fs.m, &shard_, xs, grad_dst, geo_.ld, vsums, fs.data, stream_);
+        else fs.df2(&shard_, xs, grad_dst, vsums, fs.data, stream_);
+        cb_seconds_ += wall_seconds() - t0;
+        NB_CUDA(cudaGetLastError());
+    }
     for (unsigned r = 0; r < fs.m; ++r) pend2_[index + r] = &fs;
     pend2_any_ = true;
+    return true;
+}
+
+// A terms callback (nlopt_b200_dtfunc): the user fills the library's [m][ld] terms buffer on the stream, then
+// terms_group_kernel + fold_groups_mkernel reduce each row into its 8 virtual-shard slots at vsums (row i at vsums + 8 i)
+// in the order of the __device__ functors' kernels.  One buffer serves every terms callback of the backend: each
+// callback's reduction is enqueued before the next callback can write it.
+bool DeviceBackend::reduce_terms(const FuncSpec &fs, const double *xs, double *grad_dst, double *vsums)
+{
+    if (fs.m > 65535) return fail("a terms callback takes at most 65535 rows (one grid row of the reduction each)");
+    if (!terms_) {
+        const size_t groups = shard_.groups_local ? shard_.groups_local : 1;
+        if (!small_dev((void **) &terms_, (size_t) terms_rows_ * geo_.ld * sizeof(double))) return false;
+        if (!small_dev((void **) &terms_part_, (size_t) terms_rows_ * groups * sizeof(double))) return false;
+    }
+    const double t0 = wall_seconds();
+    fs.dtf(fs.m, &shard_, xs, grad_dst, geo_.ld, terms_, fs.data, stream_);
+    cb_seconds_ += wall_seconds() - t0;
+    NB_CUDA(cudaGetLastError());
+    if (shard_.groups_local == 0) return true;              // a rank without variables: its slots stay +0.0
+    terms_group_kernel<<<dim3(shard_.groups_local, fs.m), kTermsThreads, 0, stream_>>>(shard_, terms_, geo_.ld, terms_part_);
+    nlopt_b200::detail::fold_groups_mkernel<<<dim3(shard_.local_vshards, fs.m), kTermsThreads, 0, stream_>>>(
+        terms_part_, shard_.groups_local, shard_.groups_per_vshard, vsums + shard_.vshard0);
+    stats_->kernel_launches += 2;
+    NB_CUDA(cudaGetLastError());
     return true;
 }
 
@@ -951,7 +994,7 @@ bool DeviceBackend::finish_evals(double *fvalue, double *cvalues)
             const FuncSpec *fs = pend2_[i];
             step = 1;
             if (!fs) continue;
-            if (fs->dmf2) {            // a vector constraint: its m rows, one finish call (never the objective's slot 0)
+            if (fs->dmfin) {           // a vector constraint: its m rows, one finish call (never the objective's slot 0)
                 step = fs->m;
                 if (!cvalues) continue;
                 std::vector<double> tots(fs->m);

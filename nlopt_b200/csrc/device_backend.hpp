@@ -47,6 +47,7 @@ public:
     bool finish_evals(double *fvalue, double *cvalues) override;
     bool agree_any(bool local) override;
     bool enqueue_df2(const FuncSpec &fs, Slot slot, double *grad_dst, unsigned index);
+    bool reduce_terms(const FuncSpec &fs, const double *xs, double *grad_dst, double *vsums);
     bool ensure_halo(Slot slot);
     bool eval_sharded(const FuncSpec &fs, Slot slot, double *grad_dst, unsigned index, double *value);
     bool eval_user_objective(Slot slot, bool want_grad, double *value);
@@ -188,6 +189,10 @@ private:
     size_t vs2_cap_ = 0;
     std::vector<const FuncSpec *> pend2_;
     bool pend2_any_ = false;
+    // terms callbacks (nlopt_b200_dtfunc): [terms_rows_][ld] terms, shared by every terms callback of a point (stream
+    // order), and their [terms_rows_][groups_local] group sums
+    unsigned terms_rows_ = 0;                        // max m over the terms callbacks, 0: none
+    double *terms_ = nullptr, *terms_part_ = nullptr;
     nlopt_b200_shard shard_{};
     double *halo_edges_ = nullptr;
     const double *halo_ptr_ = nullptr;

@@ -300,6 +300,7 @@ static nlopt_result set_objective(nlopt_opt opt, nlopt_func f, nlopt_b200_dfunc 
     opt->df = df;
     opt->df2 = nullptr;
     opt->dfin = nullptr;
+    opt->dtf = nullptr;
     opt->halo = 0;
     opt->sf = nullptr;
     opt->f_data = data;
@@ -343,6 +344,22 @@ nlopt_result nlopt_b200_set_min_objective_device2(nlopt_opt opt, nlopt_b200_dfun
 { return set_objective_device2(opt, f, fin, d, halo, 0); }
 nlopt_result nlopt_b200_set_max_objective_device2(nlopt_opt opt, nlopt_b200_dfunc2 f, nlopt_b200_dfinish fin, void *d, int halo)
 { return set_objective_device2(opt, f, fin, d, halo, 1); }
+
+static nlopt_result set_objective_terms(nlopt_opt opt, nlopt_b200_dtfunc f, nlopt_b200_dfinish fin, void *d, int halo,
+                                        int maximize)
+{
+    if (!f || !fin || halo < 0 || halo > 1) return NLOPT_INVALID_ARGS;
+    nlopt_result r = set_objective(opt, nullptr, df2_marker, nullptr, d, maximize);
+    if (r < 0) return r;
+    opt->dtf = f;
+    opt->dfin = fin;
+    opt->halo = halo;
+    return r;
+}
+nlopt_result nlopt_b200_set_min_objective_terms(nlopt_opt opt, nlopt_b200_dtfunc f, nlopt_b200_dfinish fin, void *d, int halo)
+{ return set_objective_terms(opt, f, fin, d, halo, 0); }
+nlopt_result nlopt_b200_set_max_objective_terms(nlopt_opt opt, nlopt_b200_dtfunc f, nlopt_b200_dfinish fin, void *d, int halo)
+{ return set_objective_terms(opt, f, fin, d, halo, 1); }
 
 static nlopt_result set_objective_sharded(nlopt_opt opt, nlopt_b200_sfunc f, void *d, int maximize)
 {
@@ -587,6 +604,45 @@ nlopt_result nlopt_b200_add_inequality_mconstraint_device2(nlopt_opt opt, unsign
 nlopt_result nlopt_b200_add_equality_mconstraint_device2(nlopt_opt opt, unsigned m, nlopt_b200_dmfunc2 h,
                                                          nlopt_b200_dmfinish fin, void *d, const double *tol, int halo)
 { return add_device_m(opt, true, m, h, fin, d, tol, halo); }
+
+// per-variable terms (nlopt_b200_dtfunc): the scalar forms check and register like the _device2 twins, the vector forms
+// like the _mconstraint_device2 twins; the callback goes in dtf, the finish in dfin / dmfin
+static nlopt_result add_terms(nlopt_opt opt, bool equality, nlopt_b200_dtfunc fc, nlopt_b200_dfinish fin, void *d, double tol,
+                              int halo)
+{
+    if (!fc || !fin || halo < 0 || halo > 1) return NLOPT_INVALID_ARGS;
+    nlopt_result r = add_any(opt, equality, false, 1, nullptr, nullptr, df2_marker, nullptr, d, &tol);
+    if (r < 0) return r;
+    nb200::ConstraintRec &c = (equality ? opt->h : opt->fc).back();
+    c.dtf = fc;
+    c.dfin = fin;
+    c.halo = halo;
+    return r;
+}
+static nlopt_result add_terms_m(nlopt_opt opt, bool equality, unsigned m, nlopt_b200_dtfunc fc, nlopt_b200_dmfinish fin,
+                                void *d, const double *tol, int halo)
+{
+    if (m && (!fc || !fin || halo < 0 || halo > 1)) return NLOPT_INVALID_ARGS;
+    nlopt_result r = add_any(opt, equality, true, m, nullptr, nullptr, df2_marker, nullptr, d, tol);
+    if (r < 0 || !m) return r;
+    nb200::ConstraintRec &c = (equality ? opt->h : opt->fc).back();
+    c.dtf = fc;
+    c.dmfin = fin;
+    c.halo = halo;
+    return r;
+}
+nlopt_result nlopt_b200_add_inequality_constraint_terms(nlopt_opt opt, nlopt_b200_dtfunc fc, nlopt_b200_dfinish fin, void *d,
+                                                        double tol, int halo)
+{ return add_terms(opt, false, fc, fin, d, tol, halo); }
+nlopt_result nlopt_b200_add_equality_constraint_terms(nlopt_opt opt, nlopt_b200_dtfunc h, nlopt_b200_dfinish fin, void *d,
+                                                      double tol, int halo)
+{ return add_terms(opt, true, h, fin, d, tol, halo); }
+nlopt_result nlopt_b200_add_inequality_mconstraint_terms(nlopt_opt opt, unsigned m, nlopt_b200_dtfunc fc,
+                                                         nlopt_b200_dmfinish fin, void *d, const double *tol, int halo)
+{ return add_terms_m(opt, false, m, fc, fin, d, tol, halo); }
+nlopt_result nlopt_b200_add_equality_mconstraint_terms(nlopt_opt opt, unsigned m, nlopt_b200_dtfunc h,
+                                                       nlopt_b200_dmfinish fin, void *d, const double *tol, int halo)
+{ return add_terms_m(opt, true, m, h, fin, d, tol, halo); }
 
 /* ------------------------------------------------------------------ stopping criteria (options.c:661-816) */
 
@@ -997,6 +1053,7 @@ nlopt_result run_ccsa(nlopt_opt opt, double *x_host, double *x_dev, double *minf
     cfg.objective.df = opt->df;
     cfg.objective.df2 = opt->df2;
     cfg.objective.dfin = opt->dfin;
+    cfg.objective.dtf = opt->dtf;
     cfg.objective.halo = opt->halo;
     cfg.objective.sf = opt->sf;
     cfg.objective.data = opt->f_data;
@@ -1006,7 +1063,7 @@ nlopt_result run_ccsa(nlopt_opt opt, double *x_host, double *x_dev, double *minf
     for (const auto &c : opt->fc) {
         nb200::FuncSpec s;
         s.m = c.m; s.f = c.f; s.mf = c.mf; s.df = c.df; s.df2 = c.df2; s.dfin = c.dfin; s.dmf2 = c.dmf2; s.dmfin = c.dmfin;
-        s.halo = c.halo; s.sf = c.sf; s.data = c.f_data;
+        s.dtf = c.dtf; s.halo = c.halo; s.sf = c.sf; s.data = c.f_data;
         cfg.constraints.push_back(s);
         tol.insert(tol.end(), c.tol.begin(), c.tol.end());
     }
@@ -1451,7 +1508,7 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
     auto to_spec = [](const nb200::ConstraintRec &c) {
         nb200::FuncSpec s;
         s.m = c.m; s.f = c.f; s.mf = c.mf; s.df = c.df; s.df2 = c.df2; s.dfin = c.dfin; s.dmf2 = c.dmf2; s.dmfin = c.dmfin;
-        s.halo = c.halo; s.data = c.f_data;
+        s.dtf = c.dtf; s.halo = c.halo; s.data = c.f_data;
         return s;
     };
     for (const auto &c : opt->h) pen.eq.push_back(to_spec(c));
@@ -1469,6 +1526,7 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
     sub->df = opt->df;
     sub->df2 = opt->df2;
     sub->dfin = opt->dfin;
+    sub->dtf = opt->dtf;
     sub->halo = opt->halo;
     sub->pre = nullptr;
     sub->maximize = 0;
@@ -1490,7 +1548,9 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
     }
     for (const auto &c : sub_fc) {
         nlopt_result r = c.dmf2 ? nlopt_b200_add_inequality_mconstraint_device2(sub, c.m, c.dmf2, c.dmfin, c.f_data, c.tol.data(), c.halo)
-                       : c.df2 ? nlopt_b200_add_inequality_constraint_device2(sub, c.df2, c.dfin, c.f_data, c.tol[0], c.halo)
+                       : c.dtf && c.dmfin ? nlopt_b200_add_inequality_mconstraint_terms(sub, c.m, c.dtf, c.dmfin, c.f_data, c.tol.data(), c.halo)
+                       : c.dtf ? nlopt_b200_add_inequality_constraint_terms(sub, c.dtf, c.dfin, c.f_data, c.tol[0], c.halo)
+                       : c.df2 ?nlopt_b200_add_inequality_constraint_device2(sub, c.df2, c.dfin, c.f_data, c.tol[0], c.halo)
                        : c.df  ? nlopt_b200_add_inequality_constraint_device(sub, c.df, c.f_data, c.tol[0])
                        : c.f   ? nlopt_add_inequality_constraint(sub, c.f, c.f_data, c.tol[0])
                                : nlopt_add_inequality_mconstraint(sub, c.m, c.mf, c.f_data, c.tol.data());
@@ -1506,7 +1566,7 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
         vc.values_only = true;
         vc.n = n;
         vc.objective.f = opt->f; vc.objective.df = opt->df; vc.objective.df2 = opt->df2; vc.objective.dfin = opt->dfin;
-        vc.objective.halo = opt->halo; vc.objective.data = opt->f_data; vc.objective.negate = opt->negate != 0;
+        vc.objective.dtf = opt->dtf; vc.objective.halo = opt->halo; vc.objective.data = opt->f_data; vc.objective.negate = opt->negate != 0;
         for (const auto &c : opt->h) vc.constraints.push_back(to_spec(c));
         for (const auto &c : pen_fc) vc.constraints.push_back(to_spec(c));
         vc.lb = opt->lb.data();

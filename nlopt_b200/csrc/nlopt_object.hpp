@@ -22,6 +22,7 @@ struct ConstraintRec {
     nlopt_b200_dfinish dfin = nullptr;
     nlopt_b200_dmfunc2 dmf2 = nullptr;  // vector asynchronous form, m rows (df then holds a marker)
     nlopt_b200_dmfinish dmfin = nullptr;
+    nlopt_b200_dtfunc dtf = nullptr;    // per-variable terms, m rows (df holds a marker; finish in dfin, or dmfin for the vector form)
     int halo = 0;
     nlopt_b200_sfunc sf = nullptr;      // sharded host callback (df then holds a marker)
     nlopt_precond pre = nullptr;
@@ -44,6 +45,7 @@ struct nlopt_opt_s {
     nlopt_b200_dfunc df = nullptr;
     nlopt_b200_dfunc2 df2 = nullptr;
     nlopt_b200_dfinish dfin = nullptr;
+    nlopt_b200_dtfunc dtf = nullptr;        // per-variable terms (finish in dfin)
     int halo = 0;
     nlopt_b200_sfunc sf = nullptr;
     void *f_data = nullptr;
