@@ -35,12 +35,17 @@
 #ifndef NLOPT_B200_H
 #define NLOPT_B200_H
 
+#ifndef __CUDACC_RTC__
 #include <stddef.h>
+#endif
 
 #ifdef __cplusplus
 extern "C" {
 #endif
 
+/* Under NVRTC (the run-time compile of nlopt_b200_jit_create, which includes nlopt_b200_device_kernels.cuh) only the
+ * shard geometry below is seen: NVRTC compiles device code and takes no host declaration. */
+#ifndef __CUDACC_RTC__
 #define NLOPT_B200 1
 #define NLOPT_EXTERN(T) extern T
 #define NLOPT_STDCALL
@@ -247,6 +252,7 @@ nlopt_result nlopt_b200_add_equality_constraint_device(nlopt_opt opt, nlopt_b200
  * `halo` > 0: the callback also reads x_dev[-halo .. -1] and x_dev[n_local .. n_local + halo - 1] (stencil functions
  * such as the chained Rosenbrock function); the library fills these cells from the neighbouring ranks before the
  * callbacks of a point run.  halo <= 1 in this build. */
+#endif  /* __CUDACC_RTC__ */
 typedef struct {
     unsigned long long n, n_local, j0;          /* global size; this rank's variables [j0, j0 + n_local)          */
     unsigned long long nchunks, chunk0;         /* 512-variable chunks: all of them / first of this rank           */
@@ -254,6 +260,7 @@ typedef struct {
     unsigned vshard0, local_vshards;
     int rank, world;
 } nlopt_b200_shard;
+#ifndef __CUDACC_RTC__
 void nlopt_b200_shard_geometry(unsigned long long n, int rank, int world, nlopt_b200_shard *out);
 typedef void (*nlopt_b200_dfunc2)(const nlopt_b200_shard *shard, const double *x_dev, double *grad_dev, double *vsums_dev,
                                   void *func_data, void *cuda_stream);
@@ -317,6 +324,44 @@ nlopt_result nlopt_b200_add_inequality_mconstraint_terms(nlopt_opt opt, unsigned
 nlopt_result nlopt_b200_add_equality_mconstraint_terms(nlopt_opt opt, unsigned m, nlopt_b200_dtfunc h,
                                                        nlopt_b200_dmfinish finish, void *h_data, const double *tol,
                                                        int halo);
+/* Device functors given as SOURCE, for callers without nvcc.  nlopt_b200_jit_create compiles `source` with NVRTC
+ * (opened at the first call; libnvrtc.so.12 by soname, else from the toolkit the library was built with) for sm_90a,
+ * with -std=c++17 --fmad=false and the caller's options, together with the map kernels of
+ * include/nlopt_b200_device_kernels.cuh, whose text the library embeds (the source may include nothing else of this
+ * library; its functor is a struct of the nlopt_b200_device.cuh concept, named by `name`, with or without namespace).
+ * The registrations below launch the header's own map_group_kernel / map_group_mkernel instantiation and the same
+ * fold kernels, so values, and whole runs, have the bits of the same functor compiled by nvcc (nlopt_b200_device.cuh).
+ * Compiled images are cached per process, keyed by source, name and options.  The handle is returned even when the
+ * compile fails: nlopt_b200_jit_errmsg then says why (NULL when compiled), nlopt_b200_jit_log holds the compiler log.
+ * A functor must have m (F::m, 0 for a scalar functor) <= 16 and halo <= 1; nlopt_b200_jit_info reports them and
+ * sizeof(F) (= param_bytes).  A registration copies the `param_bytes` bytes of the functor object at `params` (its
+ * members: scalars, arrays, device pointers) and takes an optional host finish: NULL is the identity, else
+ * finish(total, finish_data) / finish(m, totals, result, finish_data) as for the _device2 forms.  NLOPT_INVALID_ARGS,
+ * with a message, for a failed handle, param_bytes != sizeof(F), a scalar functor registered with an _mconstraint form
+ * or a vector functor with the others, and a negative or NaN tolerance; then the checks of the _device2 twins.  The
+ * handle must outlive every opt that uses it (it owns the registrations).  One GPU verified. */
+typedef struct nlopt_b200_jit_s *nlopt_b200_jit;
+nlopt_b200_jit nlopt_b200_jit_create(const char *source, const char *name, const char *const *options, int noptions);
+void nlopt_b200_jit_destroy(nlopt_b200_jit h);
+const char *nlopt_b200_jit_errmsg(nlopt_b200_jit h);
+const char *nlopt_b200_jit_log(nlopt_b200_jit h);
+/* 0, and m / halo / sizeof(F), for a compiled handle; -1 for a failed one */
+int nlopt_b200_jit_info(nlopt_b200_jit h, int *m, int *halo, size_t *param_bytes);
+/* the compiled sm_90a cubin (NULL for a failed handle) */
+const void *nlopt_b200_jit_image(nlopt_b200_jit h, size_t *bytes);
+nlopt_result nlopt_b200_jit_set_min_objective(nlopt_opt opt, nlopt_b200_jit f, const void *params, size_t param_bytes,
+                                              nlopt_b200_dfinish finish, void *finish_data);
+nlopt_result nlopt_b200_jit_set_max_objective(nlopt_opt opt, nlopt_b200_jit f, const void *params, size_t param_bytes,
+                                              nlopt_b200_dfinish finish, void *finish_data);
+nlopt_result nlopt_b200_jit_add_inequality_constraint(nlopt_opt opt, nlopt_b200_jit fc, const void *params, size_t param_bytes,
+                                                      nlopt_b200_dfinish finish, void *finish_data, double tol);
+nlopt_result nlopt_b200_jit_add_equality_constraint(nlopt_opt opt, nlopt_b200_jit h, const void *params, size_t param_bytes,
+                                                    nlopt_b200_dfinish finish, void *finish_data, double tol);
+/* tol: m entries, or NULL for zeros */
+nlopt_result nlopt_b200_jit_add_inequality_mconstraint(nlopt_opt opt, nlopt_b200_jit fc, const void *params, size_t param_bytes,
+                                                       nlopt_b200_dmfinish finish, void *finish_data, const double *tol);
+nlopt_result nlopt_b200_jit_add_equality_mconstraint(nlopt_opt opt, nlopt_b200_jit h, const void *params, size_t param_bytes,
+                                                     nlopt_b200_dmfinish finish, void *finish_data, const double *tol);
 /* Sharded HOST callbacks (one process per GPU): the callback sees only this rank's variables -- x_shard and grad_shard
  * hold the n_local entries starting at global index j0 -- and returns its ADDITIVE contribution to the function value
  * (a constant term is added by one rank only, e.g. the one with j0 == 0); the library sums the contributions over the
@@ -421,6 +466,8 @@ void nlopt_b200_release_cached_memory(void);
 /* library / device probe: returns number of visible CUDA devices, <0 on CUDA error */
 int nlopt_b200_device_count(void);
 const char *nlopt_b200_build_info(void);
+
+#endif  /* __CUDACC_RTC__ */
 
 #ifdef __cplusplus
 }

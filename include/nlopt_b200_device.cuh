@@ -54,13 +54,12 @@
 
 #include <cuda_runtime.h>
 
-#include "nlopt_b200.h"
+#include "nlopt_b200_device_kernels.cuh"
 
 namespace nlopt_b200 {
 
 namespace detail {
 
-constexpr int kThreads = 256;
 constexpr int kBlocks = 1056;            // 8 CTAs per SM on a 132-SM H100
 
 struct Workspace {
@@ -84,19 +83,6 @@ inline Workspace &workspace()
         cudaDeviceSynchronize();
     }
     return w;
-}
-
-__device__ __forceinline__ double block_sum(double v, double *smem)
-{
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) v = __dadd_rn(v, __shfl_xor_sync(0xffffffffu, v, off));
-    if ((threadIdx.x & 31) == 0) smem[threadIdx.x >> 5] = v;
-    __syncthreads();
-    double s = 0.0;
-    if (threadIdx.x == 0)
-        for (int w = 0; w < kThreads / 32; ++w) s = __dadd_rn(s, smem[w]);
-    __syncthreads();
-    return s;                            // valid in thread 0
 }
 
 template <class F>
@@ -159,89 +145,6 @@ inline double *partials2(unsigned groups)
     return w.partials;
 }
 
-// one CTA per group: thread t takes variables lo + t, lo + t + 256, ... of the group
-template <class F>
-__global__ void __launch_bounds__(kThreads) map_group_kernel(F f, nlopt_b200_shard sh, const double *x, double *grad, double *partials)
-{
-    __shared__ double smem[kThreads / 32];
-    const unsigned g = sh.group0 + blockIdx.x;
-    const unsigned long long c_lo = (unsigned long long) g * sh.nchunks / sh.groups_total - sh.chunk0;
-    const unsigned long long c_hi = (unsigned long long) (g + 1) * sh.nchunks / sh.groups_total - sh.chunk0;
-    long long lo = (long long) (c_lo * 512), hi = (long long) (c_hi * 512);
-    if (hi > (long long) sh.n_local) hi = (long long) sh.n_local;
-    double acc = 0.0;
-    for (long long jl = lo + threadIdx.x; jl < hi; jl += kThreads)
-        acc = __dadd_rn(acc, f(sh.j0 + (unsigned long long) jl, sh.n, jl, (long long) sh.n_local, x, grad ? grad + jl : nullptr));
-    const double s = block_sum(acc, smem);
-    if (threadIdx.x == 0) partials[blockIdx.x] = s;
-}
-
-// one CTA per local virtual shard: its P group sums in a fixed order
-__global__ void __launch_bounds__(kThreads) fold_groups_kernel(const double *partials, unsigned P, double *vsums /* at vshard0 */)
-{
-    __shared__ double smem[kThreads / 32];
-    const double *base = partials + (size_t) blockIdx.x * P;
-    double acc = 0.0;
-    for (unsigned r = threadIdx.x; r < P; r += kThreads) acc = __dadd_rn(acc, base[r]);
-    const double s = block_sum(acc, smem);
-    if (threadIdx.x == 0) vsums[blockIdx.x] = s;
-}
-
-// ---- vector functors (nlopt_b200_dmfunc2): F::m components from one visit of each variable ---------------------
-// map_group_mkernel is map_group_kernel with F::m accumulators per thread: the same thread->variable map, every term
-// added with __dadd_rn from +0.0, and each component reduced by block_sum's tree (xor butterfly 16..1, then the 8 warp
-// sums in warp order from +0.0; thread i does the final adds of component i).  So component i ends in the same bits
-// as a scalar functor whose terms are component i's terms.  Group sums go out as [m][groups_local].
-template <class F>
-__global__ void __launch_bounds__(kThreads) map_group_mkernel(F f, nlopt_b200_shard sh, const double *x, double *grad,
-                                                              long long grad_ld, double *partials)
-{
-    constexpr int M = F::m;
-    __shared__ double smem[M][kThreads / 32];
-    const unsigned g = sh.group0 + blockIdx.x;
-    const unsigned long long c_lo = (unsigned long long) g * sh.nchunks / sh.groups_total - sh.chunk0;
-    const unsigned long long c_hi = (unsigned long long) (g + 1) * sh.nchunks / sh.groups_total - sh.chunk0;
-    long long lo = (long long) (c_lo * 512), hi = (long long) (c_hi * 512);
-    if (hi > (long long) sh.n_local) hi = (long long) sh.n_local;
-    double acc[M];
-#pragma unroll
-    for (int i = 0; i < M; ++i) acc[i] = 0.0;
-    for (long long jl = lo + threadIdx.x; jl < hi; jl += kThreads) {
-        double t[M];
-        f(sh.j0 + (unsigned long long) jl, sh.n, jl, (long long) sh.n_local, x, t, grad ? grad + jl : nullptr, grad_ld);
-#pragma unroll
-        for (int i = 0; i < M; ++i) acc[i] = __dadd_rn(acc[i], t[i]);
-    }
-#pragma unroll
-    for (int i = 0; i < M; ++i) {
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) acc[i] = __dadd_rn(acc[i], __shfl_xor_sync(0xffffffffu, acc[i], off));
-    }
-    if ((threadIdx.x & 31) == 0) {
-#pragma unroll
-        for (int i = 0; i < M; ++i) smem[i][threadIdx.x >> 5] = acc[i];
-    }
-    __syncthreads();
-    if (threadIdx.x < M) {
-        double s = 0.0;
-        for (int w = 0; w < kThreads / 32; ++w) s = __dadd_rn(s, smem[threadIdx.x][w]);
-        partials[(size_t) threadIdx.x * gridDim.x + blockIdx.x] = s;
-    }
-}
-
-// fold_groups_kernel for every row: CTA (v, i) folds the P group sums of local virtual shard v of row i in the same
-// fixed order; row i of the partials starts at partials + i * groups_local, of the sums at vsums + 8 i
-__global__ void __launch_bounds__(kThreads) fold_groups_mkernel(const double *partials, unsigned groups_local, unsigned P,
-                                                                double *vsums /* row 0 at vshard0 */)
-{
-    __shared__ double smem[kThreads / 32];
-    const double *base = partials + (size_t) blockIdx.y * groups_local + (size_t) blockIdx.x * P;
-    double acc = 0.0;
-    for (unsigned r = threadIdx.x; r < P; r += kThreads) acc = __dadd_rn(acc, base[r]);
-    const double s = block_sum(acc, smem);
-    if (threadIdx.x == 0) vsums[(size_t) blockIdx.y * 8 + blockIdx.x] = s;
-}
-
 template <class F>
 void mtrampoline2(unsigned /* = F::m, registered by the front ends below */, const nlopt_b200_shard *sh, const double *x_dev,
                   double *grad_dev, unsigned long long grad_ld, double *vsums_dev, void *data, void *stream)
@@ -260,11 +163,6 @@ void mfinish2(unsigned, const double *totals, double *result, void *data)
 {
     static_cast<const F *>(data)->finish(totals, result);
 }
-
-template <class F, class = void>
-struct halo_of { static constexpr int value = 0; };
-template <class F>
-struct halo_of<F, decltype((void) F::halo)> { static constexpr int value = F::halo; };
 
 template <class F>
 void trampoline2(const nlopt_b200_shard *sh, const double *x_dev, double *grad_dev, double *vsums_dev, void *data, void *stream)

@@ -68,6 +68,49 @@ class _DeviceArray:
                                          "version": 2}
 
 
+class CompileError(RuntimeError):
+    """a CudaFunctor that did not compile or is not accepted; .log holds the compiler log"""
+
+    def __init__(self, msg, log=""):
+        super().__init__(msg)
+        self.log = log
+
+
+class CudaFunctor:
+    """A __device__ functor given as source (the concept of include/nlopt_b200_device.cuh), compiled at run time by
+    NVRTC for sm_90a with the library's map kernels, no nvcc needed.  `name` names the functor struct in `source`;
+    `options` are extra NVRTC options.  .m (0 for a scalar functor), .halo, .param_bytes (sizeof the functor) and .log
+    (the compiler's log).  Raises CompileError, with the compiler's message, when the source does not compile or the
+    functor is not accepted (m > 16, halo > 1).  Compiled images are cached per process."""
+
+    def __init__(self, source, name, options=(), library: Library | None = None):
+        self._lib = library or default_library()
+        opts = [o.encode() for o in options]
+        arr = (C.c_char_p * max(len(opts), 1))(*opts)
+        self._h = self._lib.nlopt_b200_jit_create(source.encode(), name.encode(), arr, len(opts))
+        if not self._h:
+            raise MemoryError("nlopt_b200_jit_create")
+        log = self._lib.nlopt_b200_jit_log(self._h)
+        self.log = log.decode(errors="replace") if log else ""
+        err = self._lib.nlopt_b200_jit_errmsg(self._h)
+        if err:
+            raise CompileError(err.decode(errors="replace"), self.log)
+        m, halo, nbytes = C.c_int(), C.c_int(), C.c_size_t()
+        self._lib.nlopt_b200_jit_info(self._h, C.byref(m), C.byref(halo), C.byref(nbytes))
+        self.m, self.halo, self.param_bytes = m.value, halo.value, nbytes.value
+
+    def image(self):
+        """the compiled sm_90a cubin"""
+        n = C.c_size_t()
+        p = self._lib.nlopt_b200_jit_image(self._h, C.byref(n))
+        return C.string_at(p, n.value) if p else b""
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            self._lib.nlopt_b200_jit_destroy(h)
+
+
 class opt:
     """One optimisation problem; thin owner of an ``nlopt_opt`` handle."""
 
@@ -316,6 +359,41 @@ class opt:
         self._check(self._lib.nlopt_b200_add_equality_mconstraint_terms(
             self._h, tol.size, self._wrap_terms(h, True, halo), self._wrap_mfinish(finish), None, _ptr(tol), int(halo)))
 
+    # ---- extension: __device__ functors given as source (CudaFunctor, nlopt_b200_jit) ---------------------------------
+    # params: the functor object's bytes (sizeof(F) of them; e.g. bytes(ctypes.Structure) or struct.pack, with
+    # tensor.data_ptr() for device arrays); finish as for the torch methods (None: the identity, applied in C).  The
+    # functor's kernels are the nvcc-built functor's kernels, so runs match it bit for bit.
+    def _cuda_reg(self, fn, f, params, finish, vector, *tail):
+        if not isinstance(f, CudaFunctor):
+            raise TypeError("expected an nlopt_b200.CudaFunctor")
+        buf = memoryview(params).tobytes()          # copied by the library at registration
+        fin = None if finish is None else (self._wrap_mfinish(finish) if vector else self._wrap_finish(finish))
+        self._keep.append(f)                    # the functor's handle owns the registration: it lives as long as this opt
+        self._check(fn(self._h, f._h, buf, len(buf), fin, None, *tail))
+
+    def set_min_objective_cuda(self, f, params=b"", finish=None):
+        self._cuda_reg(self._lib.nlopt_b200_jit_set_min_objective, f, params, finish, False)
+
+    def set_max_objective_cuda(self, f, params=b"", finish=None):
+        self._cuda_reg(self._lib.nlopt_b200_jit_set_max_objective, f, params, finish, False)
+
+    def add_inequality_constraint_cuda(self, fc, params=b"", tol=0.0, finish=None):
+        self._cuda_reg(self._lib.nlopt_b200_jit_add_inequality_constraint, fc, params, finish, False, float(tol))
+
+    def add_equality_constraint_cuda(self, h, params=b"", tol=0.0, finish=None):
+        self._cuda_reg(self._lib.nlopt_b200_jit_add_equality_constraint, h, params, finish, False, float(tol))
+
+    # m = fc.m rows; tol: m entries (None: zeros); finish maps the m totals to the m values (numpy)
+    def add_inequality_mconstraint_cuda(self, fc, params=b"", tol=None, finish=None):
+        tol = None if tol is None else _as_f64(tol, max(fc.m, 1))
+        self._cuda_reg(self._lib.nlopt_b200_jit_add_inequality_mconstraint, fc, params, finish, True,
+                       None if tol is None else _ptr(tol))
+
+    def add_equality_mconstraint_cuda(self, h, params=b"", tol=None, finish=None):
+        tol = None if tol is None else _as_f64(tol, max(h.m, 1))
+        self._cuda_reg(self._lib.nlopt_b200_jit_add_equality_mconstraint, h, params, finish, True,
+                       None if tol is None else _ptr(tol))
+
     def optimize_torch(self, x):
         """nlopt_b200_optimize_device on a torch tensor: x (contiguous float64 CUDA tensor of this rank's n_local
         variables) holds the start point on entry and the solution on return; last_optimum_value() is the optimum.
@@ -524,5 +602,5 @@ def device_count():
     return default_library().nlopt_b200_device_count()
 
 
-__all__ = ["opt", "Library", "RoundoffLimited", "ForcedStop", "algorithm_name", "device_count",
+__all__ = ["opt", "Library", "RoundoffLimited", "ForcedStop", "CudaFunctor", "CompileError", "algorithm_name", "device_count",
            "NLOPT_B200_DFUNC"] + _ALG_NAMES

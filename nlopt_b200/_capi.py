@@ -175,6 +175,23 @@ _EXT = {
         (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p, c_double_p, C.c_int]),
     "nlopt_b200_add_equality_mconstraint_terms":
         (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p, c_double_p, C.c_int]),
+    # __device__ functors given as source, compiled at run time (nlopt_b200_jit)
+    "nlopt_b200_jit_create": (C.c_void_p, [C.c_char_p, C.c_char_p, C.POINTER(C.c_char_p), C.c_int]),
+    "nlopt_b200_jit_destroy": (None, [C.c_void_p]),
+    "nlopt_b200_jit_errmsg": (C.c_char_p, [C.c_void_p]),
+    "nlopt_b200_jit_log": (C.c_char_p, [C.c_void_p]),
+    "nlopt_b200_jit_info": (C.c_int, [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_size_t)]),
+    "nlopt_b200_jit_image": (C.c_void_p, [C.c_void_p, C.POINTER(C.c_size_t)]),
+    "nlopt_b200_jit_set_min_objective": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    "nlopt_b200_jit_set_max_objective": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    "nlopt_b200_jit_add_inequality_constraint":
+        (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_double]),
+    "nlopt_b200_jit_add_equality_constraint":
+        (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_double]),
+    "nlopt_b200_jit_add_inequality_mconstraint":
+        (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, c_double_p]),
+    "nlopt_b200_jit_add_equality_mconstraint":
+        (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, c_double_p]),
     "nlopt_b200_shard_geometry": (None, [C.c_ulonglong, C.c_int, C.c_int, C.c_void_p]),
     "nlopt_b200_set_min_objective_sharded": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "nlopt_b200_add_inequality_constraint_sharded": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_double]),

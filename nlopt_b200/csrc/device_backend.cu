@@ -950,6 +950,18 @@ bool DeviceBackend::reduce_terms(const FuncSpec &fs, const double *xs, double *g
     return true;
 }
 
+// The fold of nlopt_b200_device.cuh's trampoline2 (m == 0) / mtrampoline2 (m rows) for the functors compiled at run
+// time (jit.cu): the header's fold kernels are defined in this translation unit, and a second one may not define them.
+void fold_functor_sums(unsigned m, const double *partials, const nlopt_b200_shard &sh, double *vsums, cudaStream_t s)
+{
+    if (m == 0)
+        nlopt_b200::detail::fold_groups_kernel<<<sh.local_vshards, nlopt_b200::detail::kThreads, 0, s>>>(
+            partials, sh.groups_per_vshard, vsums + sh.vshard0);
+    else
+        nlopt_b200::detail::fold_groups_mkernel<<<dim3(sh.local_vshards, m), nlopt_b200::detail::kThreads, 0, s>>>(
+            partials, sh.groups_local, sh.groups_per_vshard, vsums + sh.vshard0);
+}
+
 // The halo cells of the slot's x for stencil callbacks: once per point (x_epoch_), only with several ranks.
 bool DeviceBackend::ensure_halo(Slot slot)
 {
