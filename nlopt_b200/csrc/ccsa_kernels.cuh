@@ -582,7 +582,8 @@ __device__ __forceinline__ void fold_init(double *s_w)
 
 template <int NV>
 __device__ __forceinline__ void fold_generation(const double *grouptags, unsigned ngroups, unsigned P, unsigned local_vshards,
-                                                unsigned long long tag, int k0, int nk, double *s_w, double *s_vs)
+                                                unsigned long long tag, int k0, int nk, double *s_w, double *s_vs,
+                                                bool reverse = false)
 {
     const int lane = threadIdx.x & 31;
     const int sub = threadIdx.x >> 5;
@@ -590,7 +591,10 @@ __device__ __forceinline__ void fold_generation(const double *grouptags, unsigne
     const unsigned fw_per = fw_all < (unsigned) kGroupWarps ? fw_all : (unsigned) kGroupWarps;      // non-empty fold warps per shard
     const unsigned nitems = local_vshards * fw_per;
     // (Polling two items per round trip was tried and measured slower.)
-    for (unsigned item = sub; item < nitems; item += kGroupWarps) {
+    // reverse: the items are polled last shard first, for generations whose groups were claimed in descending order.
+    // Each item writes its own slot of s_w, so the order in which they are polled does not change a bit.
+    for (unsigned i = sub; i < nitems; i += kGroupWarps) {
+        const unsigned item = reverse ? nitems - 1 - i : i;
         const unsigned v = item / fw_per, w = item % fw_per;
         double acc[NV];
 #pragma unroll
@@ -1344,7 +1348,9 @@ __global__ void __launch_bounds__(kBlock, 2) dual_eval_wide_kernel(const __grid_
 // Timeline instrumentation (tools/trace_solve.py builds a separate library with -DNB200_TRACE; the product build
 // contains none of it).  Per generation g, 16 counters at trace[16 g]: 0 published | 1 ~min / 2 max "CTA saw it" |
 // 3 ~min / 4 max "group record stored" | 5 all shard sums in | 6 totals ready | 7 optimiser done | 8 sum / 9 count
-// of per-group sweep times.  Row 0 holds the CTA start times.  All in %globaltimer nanoseconds.
+// of per-group sweep times | TMA-staged form only: 10 ~min / 11 max "a CTA stored its last group record of g",
+// 12 max / 13 ~min "a producer found its ring full of g's chunks while its consumers wait for g's multipliers".
+// Row 0 holds the CTA start times.  All in %globaltimer nanoseconds.
 #ifdef NB200_TRACE
 constexpr int kTraceGens = 512;
 #define NB_TR(...) __VA_ARGS__
@@ -1542,8 +1548,10 @@ struct SharedMultipliers {                // what the point functions read in th
 // The folder CTA's loop (kept out of line so that its registers do not weigh on the sweep loop).
 // s_vs [8 x NV] (the shard sums of the generation in flight) and s_w [8 x 8 x NV] (per shard: the 8 fold-warp results)
 // are provided by the caller: the TMA-staged kernel's folder CTA lends its (otherwise unused) stage ring.
+// serp: the sweepers claim the groups of even generations in descending order (dual_solve_tma_kernel); the folder
+// polls the shards of those generations in the same order.
 template <int NV>
-__device__ __noinline__ void solve_folder(const SolveArgs &sa, double *s_vs, double *s_w, void *mach_storage)
+__device__ __noinline__ void solve_folder(const SolveArgs &sa, double *s_vs, double *s_w, void *mach_storage, bool serp = false)
 {
     const DualArgs &a = sa.d;
     SolveState *st = sa.st;
@@ -1592,7 +1600,7 @@ __device__ __noinline__ void solve_folder(const SolveArgs &sa, double *s_vs, dou
     if (s_exit) return;
     for (unsigned long long gen = 1;; ++gen) {
         const unsigned long long tag = sa.tag0 | gen;
-        fold_generation<NV>(a.grouptags, ngroups, a.segs_per_vshard, a.local_vshards, tag, 0, NV, s_w, s_vs);
+        fold_generation<NV>(a.grouptags, ngroups, a.segs_per_vshard, a.local_vshards, tag, 0, NV, s_w, s_vs, serp && !(gen & 1));
         // ---- warp 0: totals (exchange if sharded), the dual optimiser's turn, publication ----
         if (sub == 0) {
             NB_TR(if (lane == 0 && gen < kTraceGens) sa.trace[16 * gen + 5] = nb_globaltimer();)
@@ -1990,7 +1998,7 @@ __global__ void __launch_bounds__(kBlock, MINB) dual_solve_async_kernel(const __
 // steps the dual optimiser and publishes y_{g+1}, every sweeper's ring fills with the first chunks of generation g + 1;
 // when y arrives the consumers start from shared memory and the producer keeps STAGES chunks in flight behind them.
 //   producer (warp 8, one thread): claims groups from the same monotonic counter as the register form (claim c ->
-//     generation c / ngroups + 1, group c % ngroups), and for every chunk waits for a free stage, writes the stage's
+//     generation c / ngroups + 1, group c % ngroups, counted down on even generations), and for every chunk waits for a free stage, writes the stage's
 //     metadata {generation, group, first/last chunk, pair offset}, arms the "full" barrier and issues the bulk loads.
 //   consumers (warps 0-7): follow the stage metadata -- first chunk of a group in a new generation: wait for that
 //     generation's multipliers (warp 0 polls the tagged slots, as in the register form); every chunk: operands from
@@ -2043,6 +2051,7 @@ __global__ void __launch_bounds__(kTmaBlock, MINB) dual_solve_tma_kernel(const _
     __shared__ int s_store, s_exit;
     __shared__ volatile int s_stop, s_prod_done;
     __shared__ volatile unsigned long long s_issued;
+    NB_TR(__shared__ volatile unsigned long long s_park_gen;)   // generation whose multipliers warp 0 is polling for, else 0
 
     const int lane = threadIdx.x & 31;
     const int warp = threadIdx.x >> 5;
@@ -2051,7 +2060,7 @@ __global__ void __launch_bounds__(kTmaBlock, MINB) dual_solve_tma_kernel(const _
         static_assert((size_t) STAGES * NARR * kChunkBytes >= (size_t) (kVirtualShards * NV + kVirtualShards * kGroupWarps * NV) * sizeof(double), "fold scratch fits the ring");
         constexpr size_t kFoldDoubles = (size_t) kVirtualShards * NV + (size_t) kVirtualShards * kGroupWarps * NV;
         static_assert((size_t) STAGES * NARR * kChunkBytes >= kFoldDoubles * sizeof(double) + 32 * sizeof(WarpDualMachine<NV - 3>) + 16, "fold scratch + optimiser state fit the ring");
-        if (warp < kGroupWarps) solve_folder<NV>(sa, scratch, scratch + kVirtualShards * NV, scratch + ((kFoldDoubles + 1) & ~(size_t) 1));
+        if (warp < kGroupWarps) solve_folder<NV>(sa, scratch, scratch + kVirtualShards * NV, scratch + ((kFoldDoubles + 1) & ~(size_t) 1), true);
         return;
     }
     const DualArgs &a = sa.d;
@@ -2064,7 +2073,7 @@ __global__ void __launch_bounds__(kTmaBlock, MINB) dual_solve_tma_kernel(const _
             mbar_init(&s_empty[st], kGroupWarps);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        s_exit = 0; s_store = 0; s_stop = 0; s_prod_done = 0; s_issued = 0ull;
+        s_exit = 0; s_store = 0; s_stop = 0; s_prod_done = 0; s_issued = 0ull; NB_TR(s_park_gen = 0ull;)
     }
     __syncthreads();
 
@@ -2085,13 +2094,21 @@ __global__ void __launch_bounds__(kTmaBlock, MINB) dual_solve_tma_kernel(const _
             while (!stop) {
                 const unsigned long long c = atomicAdd(&st_g->claim, 1ull);
                 const unsigned long long gen = c / ngroups + 1;
-                const unsigned gl = (unsigned) (c % ngroups);
+                // serpentine: even generations take the groups in descending order, so that a generation starts on the
+                // groups the previous one read last, which are still in the L2 (the group records, and so the sums, do
+                // not depend on the order in which the groups are swept)
+                const unsigned gl = (gen & 1) ? (unsigned) (c % ngroups) : ngroups - 1u - (unsigned) (c % ngroups);
                 unsigned long long p_lo, p_hi;
                 group_pairs(a.nchunks, a.nseg_total, a.chunk0, a.seg0 + gl, &p_lo, &p_hi);
                 const bool empty = p_lo == p_hi;
                 for (unsigned long long p = p_lo; p < p_hi || (empty && p == p_lo); p += kChunkPairs) {
-                    while (!mbar_test(&s_empty[st], phase ^ 1u))          // a fresh barrier passes at once
+                    NB_TR(bool tr_parked = false;)
+                    while (!mbar_test(&s_empty[st], phase ^ 1u)) {        // a fresh barrier passes at once
                         if (s_stop) { stop = true; break; }
+                        NB_TR(if (!tr_parked && s_park_gen == gen && gen < kTraceGens) {
+                                  tr_parked = true; const unsigned long long t = nb_globaltimer();
+                                  atomicMax(&sa.trace[16 * gen + 12], t); atomicMax(&sa.trace[16 * gen + 13], ~t); })
+                    }
                     if (stop) break;
                     StageMeta mt;
                     mt.gen = gen; mt.p = p; mt.gl = gl;
@@ -2132,6 +2149,7 @@ __global__ void __launch_bounds__(kTmaBlock, MINB) dual_solve_tma_kernel(const _
 #pragma unroll
     for (int k = 0; k < NV; ++k) acc[k] = 0.0;
     bool store = false;
+    NB_TR(unsigned long long tr_s0 = 0, tr_last = 0;)       // warp 0: start of the group in flight, time of the last record
     for (;;) {
         mbar_wait(&s_full[st], phase);                        // the stage's bytes and its metadata are visible
         const StageMeta mt = s_meta[st];
@@ -2144,6 +2162,7 @@ __global__ void __launch_bounds__(kTmaBlock, MINB) dual_solve_tma_kernel(const _
                     double v;
                     int ex = 0;
                     unsigned spins = 0;
+                    NB_TR(if (lane == 0) s_park_gen = mt.gen;)
                     for (;;) {
                         if (__all_sync(0xffffffffu, slot_get(st_g->pub + 2 * slot, tag, &v))) break;
                         if ((++spins & 7u) == 0u && __any_sync(0xffffffffu, ld_gpu_s32(&st_g->done))) {
@@ -2152,17 +2171,23 @@ __global__ void __launch_bounds__(kTmaBlock, MINB) dual_solve_tma_kernel(const _
                         }
                         __nanosleep(20);
                     }
+                    NB_TR(if (lane == 0) s_park_gen = 0ull;)
                     if (ex) s_exit = 1;
                     else if (lane < a.m) s_y[lane] = v;
                     else if (lane == a.m) s_u = v;
                     else if (lane == a.m + 1) s_store = (int) (__double_as_longlong(v) & 1ll);
                 }
                 asm volatile("bar.sync 1, %0;" ::"r"(32 * kGroupWarps) : "memory");
+                NB_TR(if (threadIdx.x == 0) {
+                          const unsigned long long t = nb_globaltimer();
+                          if (my_gen && my_gen < kTraceGens) { atomicMax(&sa.trace[16 * my_gen + 10], ~tr_last); atomicMax(&sa.trace[16 * my_gen + 11], tr_last); }
+                          if (!s_exit && mt.gen < kTraceGens) { atomicMax(&sa.trace[16 * mt.gen + 1], ~t); atomicMax(&sa.trace[16 * mt.gen + 2], t); } })
                 if (s_exit) break;
                 my_gen = mt.gen;
                 mu.u_ccsaq = s_u;
                 store = s_store != 0;
             }
+            NB_TR(tr_s0 = nb_globaltimer();)
 #pragma unroll
             for (int k = 0; k < NV; ++k) acc[k] = 0.0;
         }
@@ -2214,6 +2239,8 @@ __global__ void __launch_bounds__(kTmaBlock, MINB) dual_solve_tma_kernel(const _
             asm volatile("bar.sync 1, %0;" ::"r"(32 * kGroupWarps) : "memory");
             parity ^= 1;
             if (sub == 0) put_group_record<NV>(srec, a.grouptags, ngroups, mt.gl, sa.tag0 | my_gen, lane);
+            NB_TR(if (sub == 0 && lane == 0 && my_gen < kTraceGens) { const unsigned long long t = nb_globaltimer(); unsigned long long *r = sa.trace + 16 * my_gen;
+                      atomicMax(r + 3, ~t); atomicMax(r + 4, t); atomicAdd(r + 8, t - tr_s0); atomicAdd(r + 9, 1ull); tr_last = t; })
         }
     }
     // ---- leaving: stop the producer, then wait for every copy it has issued (the stage we hold is complete) ----

@@ -1489,8 +1489,10 @@ bool DeviceBackend::dual_solve(double *y, const double *lo, const double *hi, co
             for (int g = 1; g < kTraceGens && h[16 * g]; ++g) {
                 const unsigned long long *r = &h[16 * g];
                 const unsigned long long p = r[0];
-                std::fprintf(f, "  gen %d phase0 %lld phase3 %lld phase7 %lld polls_t0 %llu t0_at_barrier %lld seen[%lld..%lld] recs[%lld..%lld] rank_done %lld totals %lld machine %lld next_pub %lld | mean_group_sweep %llu ns x %llu\n", g,
-                             (long long) (r[10] - p), (long long) (r[11] - p), (long long) (r[12] - p), r[13], (long long) (r[14] - p),
+                // lastrec / parked: TMA-staged form only (0 otherwise)
+                std::fprintf(f, "  gen %d lastrec[%lld..%lld] parked[%lld..%lld] seen[%lld..%lld] recs[%lld..%lld] rank_done %lld totals %lld machine %lld next_pub %lld | mean_group_sweep %llu ns x %llu\n", g,
+                             r[11] ? (long long) (~r[10] - p) : 0ll, r[11] ? (long long) (r[11] - p) : 0ll,
+                             r[12] ? (long long) (~r[13] - p) : 0ll, r[12] ? (long long) (r[12] - p) : 0ll,
                              (long long) (~r[1] - p), (long long) (r[2] - p), (long long) (~r[3] - p), (long long) (r[4] - p),
                              (long long) (r[5] - p), (long long) (r[6] - p), (long long) (r[7] - p),
                              (long long) (h[16 * (g + 1)] ? h[16 * (g + 1)] - p : 0), r[9] ? r[8] / r[9] : 0ull, r[9]);

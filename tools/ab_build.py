@@ -17,6 +17,7 @@ def build(name, defines):
     out = os.path.join(ROOT, "build", "ab", name)
     os.makedirs(out, exist_ok=True)
     cuda_home = os.path.dirname(os.path.dirname(G.NVCC))
+    G.write_jit_headers(os.path.join(G.BUILD, "jit_headers.inc"))
     objs = []
     for src in G.LIB_SOURCES_CU:
         obj = os.path.join(out, src + ".o")
@@ -25,7 +26,8 @@ def build(name, defines):
         objs.append(obj)
     for src in G.LIB_SOURCES_CXX:
         obj = os.path.join(out, src + ".o")
-        G._run(["g++", *G.CXX_FLAGS, *defines, f"-I{cuda_home}/include", "-c", os.path.join(G.CSRC, src), "-o", obj])
+        extra = ["-I" + G.BUILD, f'-DNLOPT_B200_CUDA_LIB64="{cuda_home}/lib64"'] if src == "jit.cpp" else []      # as in build_library
+        G._run(["g++", *G.CXX_FLAGS, *extra, *defines, f"-I{cuda_home}/include", "-c", os.path.join(G.CSRC, src), "-o", obj])
         objs.append(obj)
     lib = os.path.join(out, "libnlopt_b200.so")
     G._run([G.NVCC, *G.ARCH, "-shared", "-o", lib, *objs, "-cudart", "shared", "-ldl", "-Xlinker", "-soname,libnlopt_b200.so",
