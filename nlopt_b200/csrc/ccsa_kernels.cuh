@@ -35,18 +35,6 @@
 #include "dual_mma.hpp"
 #include "pair_math.cuh"
 
-// NB200_PAIR = 1 (default): the sweep evaluates the two variables of a 128-bit load with the straight-line closed forms
-// of pair_math.cuh / mma_pair / ccsaq_pair; 0: one variable after the other through mma_point / ccsaq_point (the A/B
-// build of tools/ab_build.py).  Both give the same bits.
-#ifndef NB200_PAIR
-#define NB200_PAIR 1
-#endif
-// NB200_PRELOAD = 1 (default): the persistent solve kernel requests the first chunk of a group before it waits for the
-// generation's multipliers (load_chunk / sweep_group_preloaded); 0: loads start after the multipliers have arrived.
-#ifndef NB200_PRELOAD
-#define NB200_PRELOAD 1
-#endif
-
 namespace nb200 {
 
 constexpr int kBlock = 256;              // threads per CTA of every kernel here
@@ -86,33 +74,18 @@ __device__ __forceinline__ double2 ld_stream_pol(const double2 *p, unsigned long
     asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.f64 {%0, %1}, [%2], %3;" : "=d"(v.x), "=d"(v.y) : "l"(p), "l"(pol));
     return v;
 }
-// L1 prefetch experiment (b200_l1_prefetch): bit 31 of the mask.  The sweep then asks the L1 for the NEXT chunk of every
-// operand array (prefetch.global.L1, no register cost) while it works on the current one, and loads with L1 allocation,
-// so that the dependent load -> compute chain of a small shard finds its operands a few cycles away.
-constexpr unsigned kL1PrefetchBit = 1u << 31;
-__device__ __forceinline__ double2 ld_alloc(const double2 *p)
-{
-    double2 v;
-    asm volatile("ld.global.nc.v2.f64 {%0, %1}, [%2];" : "=d"(v.x), "=d"(v.y) : "l"(p));
-    return v;
-}
-__device__ __forceinline__ void prefetch_l1(const void *p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); }
 
 struct L2Policies {
     unsigned long long keep, stream;
     unsigned mask;                      // bit k set: operand array k (0 x, 1 lb, 2 ub, 3 sigma, 4 grad f, 5+i row i) is kept
-    bool l1pf;
     __device__ __forceinline__ void init(unsigned m)
     {
-        l1pf = (m & kL1PrefetchBit) != 0u;
-        m &= ~kL1PrefetchBit;
         mask = m;
         asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(keep));
         asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(stream));
     }
     __device__ __forceinline__ double2 ld(const double2 *p, int k) const
     {
-        if (l1pf) return ld_alloc(p);
         if (mask == 0u) return ld_stream(p);          // nothing to protect: the plain streaming load (no policy operand)
         return ld_stream_pol(p, ((mask >> k) & 1u) ? keep : stream);
     }
@@ -268,12 +241,10 @@ struct DualArgs {
     // fused cross-rank exchange over NVLink peer memory (null box[0]: NCCL path instead)
     double *box[8];               // box[r]: rank r's mailbox as mapped into this process (CUDA IPC)
     int rank, world;
-    unsigned l2_keep;             // operand arrays to hold in L2 across evaluations (L2Policies::mask)
-    unsigned prefetch_chunks;     // solve kernel: chunks of its next group a waiting sweeper asks the L2 to fetch
-    unsigned stagger_ns, sm_count;    // solve kernel: start-of-generation skew between the warps that share an SM sub-partition (0: none)
     // the multipliers and penalties
     int m;                        // total number of constraints (rows of G)
     unsigned active;              // bit i clear: constraint i switched off (MMA, NaN value)            (m <= 16)
+    unsigned l2_keep;             // operand arrays to hold in L2 across evaluations (L2Policies::mask)
     double rho, half_rho, u_ccsaq;    // u_ccsaq = rho + sum_i rhoc_i y_i (ccsa_quadratic.c:116-120)
     double y[kMaxParamM], rhoc[kMaxParamM], half_rhoc[kMaxParamM];       // (m <= 16)
     const double *wide;           // m > 16: device block  y[m] | rhoc[m] | half_rhoc[m] | active[m] (1.0 / 0.0)
@@ -700,14 +671,12 @@ __device__ __noinline__ void eval_folder(const DualArgs &a, int nv_total)
 // number of ranks -- so the m+3 sums are bit-identical for every launch geometry and every world size.
 //
 // Sweep one group: this warp's lanes of every chunk of group `gl`, m+3 lane accumulators.
-// POL: load through the per-array L2 cache policies (persistent solve kernel with b200_l2_keep_mb), else plain
-// streaming loads.
 // SB ("scalar bounds"): every lb entry equals a.lb_u and every ub entry a.ub_u (box bounds set with
 // nlopt_set_*_bounds1).  The two arrays are not read: 3 + m operand arrays per evaluation instead of 5 + m.  The
 // closed forms receive the same values as from the arrays, so the results are the same bits.
-template <int VARIANT, int MAXM, bool FULL, int UNROLL, bool POL, bool SB, class MU>
-__device__ __forceinline__ void sweep_group(const DualArgs &a, const MU &mu, const L2Policies &pol, bool store, unsigned gl, int sub,
-                                            int lane, double (&acc)[3 + (MAXM > 0 ? MAXM : 1)])
+template <int VARIANT, int MAXM, bool FULL, int UNROLL, bool SB, class MU>
+__device__ __forceinline__ void sweep_group(const DualArgs &a, const MU &mu, bool store, unsigned gl, int sub, int lane,
+                                            double (&acc)[3 + (MAXM > 0 ? MAXM : 1)])
 {
     constexpr int MR = MAXM > 0 ? MAXM : 1;
     const double2 *x2 = reinterpret_cast<const double2 *>(a.x);
@@ -717,10 +686,8 @@ __device__ __forceinline__ void sweep_group(const DualArgs &a, const MU &mu, con
     const double2 *g2 = reinterpret_cast<const double2 *>(a.g);
     unsigned long long p_lo, p_hi;
     group_pairs(a.nchunks, a.nseg_total, a.chunk0, a.seg0 + gl, &p_lo, &p_hi);
-#if NB200_PAIR
     DivBy U;
     if (VARIANT != 0) U = prep_div(mu.u());                  // CCSAQ: every variable divides by the same u
-#endif
 
     for (unsigned long long p0 = p_lo + sub * 32 + lane; p0 < p_hi; p0 += (unsigned long long) kChunkPairs * UNROLL) {
         double2 vx[UNROLL], vlb[UNROLL], vub[UNROLL], vs[UNROLL], vg[UNROLL];
@@ -736,26 +703,9 @@ __device__ __forceinline__ void sweep_group(const DualArgs &a, const MU &mu, con
                 vub[u] = make_double2(a.ub_u, a.ub_u);
             }
             if (live) {
-                if (POL && pol.l1pf && u == UNROLL - 1) {
-                    const unsigned long long pn = p + kChunkPairs;                  // this lane's pair of the next chunk
-                    if (pn < p_hi) {
-                        prefetch_l1(x2 + pn); prefetch_l1(s2v + pn); prefetch_l1(g2 + pn);
-                        if (!SB) { prefetch_l1(lb2 + pn); prefetch_l1(ub2 + pn); }
-#pragma unroll
-                        for (int i = 0; i < MR; ++i)
-                            if (MAXM > 0 && (FULL || i < mu.m))
-                                prefetch_l1(reinterpret_cast<const double2 *>(a.G + (unsigned long long) i * a.ld) + pn);
-                    }
-                }
-                if (POL) {
-                    vx[u] = pol.ld(x2 + p, 0);
-                    if (!SB) { vlb[u] = pol.ld(lb2 + p, 1); vub[u] = pol.ld(ub2 + p, 2); }
-                    vs[u] = pol.ld(s2v + p, 3); vg[u] = pol.ld(g2 + p, 4);
-                } else {
-                    vx[u] = ld_stream(x2 + p);
-                    if (!SB) { vlb[u] = ld_stream(lb2 + p); vub[u] = ld_stream(ub2 + p); }
-                    vs[u] = ld_stream(s2v + p); vg[u] = ld_stream(g2 + p);
-                }
+                vx[u] = ld_stream(x2 + p);
+                if (!SB) { vlb[u] = ld_stream(lb2 + p); vub[u] = ld_stream(ub2 + p); }
+                vs[u] = ld_stream(s2v + p); vg[u] = ld_stream(g2 + p);
             }
 #pragma unroll
             for (int i = 0; i < MR; ++i) {
@@ -763,7 +713,7 @@ __device__ __forceinline__ void sweep_group(const DualArgs &a, const MU &mu, con
                 Gb[u][i] = 0.0;
                 if (MAXM > 0 && (FULL || i < mu.m) && live) {
                     const double2 *gp = reinterpret_cast<const double2 *>(a.G + (unsigned long long) i * a.ld) + p;
-                    const double2 t = POL ? pol.ld(gp, 5 + i) : ld_stream(gp);
+                    const double2 t = ld_stream(gp);
                     Ga[u][i] = t.x;
                     Gb[u][i] = t.y;
                 }
@@ -774,22 +724,12 @@ __device__ __forceinline__ void sweep_group(const DualArgs &a, const MU &mu, con
             const unsigned long long p = p0 + (unsigned long long) kChunkPairs * u;
             const bool live = u == 0 || p < p_hi;
             double2 xc;
-#if NB200_PAIR
             if (VARIANT == 0 && kPairMMA<MAXM>) xc = mma_pair<MAXM, FULL>(mu, vx[u], vlb[u], vub[u], vs[u], vg[u], Ga[u], Gb[u], acc);
             else if (VARIANT != 0) xc = ccsaq_pair<MAXM, FULL>(mu, U, vx[u], vlb[u], vub[u], vs[u], vg[u], Ga[u], Gb[u], acc);
             else {
                 xc.x = mma_point<MAXM, FULL>(mu, vx[u].x, vlb[u].x, vub[u].x, vs[u].x, vg[u].x, Ga[u], acc);
                 xc.y = mma_point<MAXM, FULL>(mu, vx[u].y, vlb[u].y, vub[u].y, vs[u].y, vg[u].y, Gb[u], acc);
             }
-#else
-            if (VARIANT == 0) {
-                xc.x = mma_point<MAXM, FULL>(mu, vx[u].x, vlb[u].x, vub[u].x, vs[u].x, vg[u].x, Ga[u], acc);
-                xc.y = mma_point<MAXM, FULL>(mu, vx[u].y, vlb[u].y, vub[u].y, vs[u].y, vg[u].y, Gb[u], acc);
-            } else {
-                xc.x = ccsaq_point<MAXM, FULL>(mu, vx[u].x, vlb[u].x, vub[u].x, vs[u].x, vg[u].x, Ga[u], acc);
-                xc.y = ccsaq_point<MAXM, FULL>(mu, vx[u].y, vlb[u].y, vub[u].y, vs[u].y, vg[u].y, Gb[u], acc);
-            }
-#endif
             if (store && live) st_stream(reinterpret_cast<double2 *>(a.xcur) + p, xc);
         }
     }
@@ -852,22 +792,12 @@ __device__ __forceinline__ double2 compute_chunk(const MU &mu, const DivBy &U, c
                                                  double (&acc)[3 + (MAXM > 0 ? MAXM : 1)])
 {
     double2 xc;
-#if NB200_PAIR
     if (VARIANT == 0 && PAIR_MMA) xc = mma_pair<MAXM, FULL>(mu, r.x, r.lb, r.ub, r.s, r.g, r.Ga, r.Gb, acc);
     else if (VARIANT != 0) xc = ccsaq_pair<MAXM, FULL>(mu, U, r.x, r.lb, r.ub, r.s, r.g, r.Ga, r.Gb, acc);
     else {
         xc.x = mma_point<MAXM, FULL>(mu, r.x.x, r.lb.x, r.ub.x, r.s.x, r.g.x, r.Ga, acc);
         xc.y = mma_point<MAXM, FULL>(mu, r.x.y, r.lb.y, r.ub.y, r.s.y, r.g.y, r.Gb, acc);
     }
-#else
-    if (VARIANT == 0) {
-        xc.x = mma_point<MAXM, FULL>(mu, r.x.x, r.lb.x, r.ub.x, r.s.x, r.g.x, r.Ga, acc);
-        xc.y = mma_point<MAXM, FULL>(mu, r.x.y, r.lb.y, r.ub.y, r.s.y, r.g.y, r.Gb, acc);
-    } else {
-        xc.x = ccsaq_point<MAXM, FULL>(mu, r.x.x, r.lb.x, r.ub.x, r.s.x, r.g.x, r.Ga, acc);
-        xc.y = ccsaq_point<MAXM, FULL>(mu, r.x.y, r.lb.y, r.ub.y, r.s.y, r.g.y, r.Gb, acc);
-    }
-#endif
     return xc;
 }
 
@@ -879,9 +809,7 @@ __device__ __forceinline__ void sweep_group_preloaded(const DualArgs &a, const M
 {
     DivBy U;
     U.b = 1.0; U.r = 1.0; U.hb = 0x3ff00000; U.zero_ok = 1u;
-#if NB200_PAIR
     if (VARIANT != 0) U = prep_div(mu.u());                  // CCSAQ: every variable divides by the same u
-#endif
     unsigned long long p = p_first;
     bool live = p < p_hi;
     while (live) {
@@ -891,35 +819,6 @@ __device__ __forceinline__ void sweep_group_preloaded(const DualArgs &a, const M
         live = p < p_hi;
         if (live) load_chunk<MAXM, FULL, POL, SB>(a, mu.m, pol, p, true, r);
     }
-}
-
-// The operands of a sweep do not depend on the multipliers.  A sweeper of the persistent solve kernel that has to wait
-// for the next generation's multipliers first asks the L2 to fetch the head of its next group -- one bulk prefetch per
-// operand array, issued by one thread each, no registers held -- so that the serial part of a generation (last
-// record, fold, exchange, optimiser step, publication) overlaps with HBM traffic instead of leaving the memory system
-// idle: `chunks` x (5+m) x 4 KB per CTA.
-__device__ __forceinline__ void prefetch_l2_bulk(const void *p, unsigned bytes)
-{
-    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
-}
-// called by ONE thread: the bulk prefetch is a uniform-datapath instruction (UBLKPF), one array per issue
-template <bool SB>
-__device__ __forceinline__ void prefetch_group_head(const DualArgs &a, unsigned gl, unsigned chunks)
-{
-    unsigned long long p_lo, p_hi;
-    group_pairs(a.nchunks, a.nseg_total, a.chunk0, a.seg0 + gl, &p_lo, &p_hi);
-    unsigned long long np = p_hi - p_lo;
-    if (np > (unsigned long long) chunks * kChunkPairs) np = (unsigned long long) chunks * kChunkPairs;
-    if (np == 0) return;
-    const unsigned bytes = (unsigned) (np * 16);
-    prefetch_l2_bulk(a.x + 2 * p_lo, bytes);
-    if (!SB) {
-        prefetch_l2_bulk(a.lb + 2 * p_lo, bytes);
-        prefetch_l2_bulk(a.ub + 2 * p_lo, bytes);
-    }
-    prefetch_l2_bulk(a.sigma + 2 * p_lo, bytes);
-    prefetch_l2_bulk(a.g + 2 * p_lo, bytes);
-    for (int i = 0; i < a.m; ++i) prefetch_l2_bulk(a.G + (unsigned long long) i * a.ld + 2 * p_lo, bytes);
 }
 
 // group record = the 8 warp records added in warp order, dropped into the group's tagged slots
@@ -950,14 +849,12 @@ __global__ void __launch_bounds__(BLOCK, MINB) dual_eval_kernel(const __grid_con
     const unsigned nslots = gridDim.x - 1;
     const unsigned ngroups = a.segs_per_vshard * a.local_vshards;
     __shared__ double s_rec[2][kGroupWarps * NV];
-    L2Policies pol;
-    pol.init(a.l2_keep);
     int parity = 0;
     for (unsigned gl = blockIdx.x; gl < ngroups; gl += nslots) {
         double acc[NV];
 #pragma unroll
         for (int k = 0; k < NV; ++k) acc[k] = 0.0;
-        sweep_group<VARIANT, MAXM, FULL, UNROLL, false, SB>(a, a, pol, STORE, gl, sub, lane, acc);   // multipliers = the parameter block itself
+        sweep_group<VARIANT, MAXM, FULL, UNROLL, SB>(a, a, STORE, gl, sub, lane, acc);   // multipliers = the parameter block itself
 
         // warp record -> shared memory; one CTA barrier per group; the record buffer is double-buffered across
         // iterations so the next group's writers can never overtake this group's reader.
@@ -1363,19 +1260,9 @@ constexpr int kTraceGens = 512;
 // lane and every lane executes the same scalar control flow.  Sums over i are taken in index order through shuffles,
 // so every operation and its order are those of the host machine: the two produce the same bits
 // (tests/test_gpu_parity.py::test_fused_solve_equals_host_driven).
-// MAXM bounds m at compile time: with NB200_MACH_UNROLL the index-order sums over the multipliers are unrolled with a
-// predicate, so that their shuffles are issued back to back instead of one per loop trip (they sit on the serial path
-// of every generation).
-#ifndef NB200_MACH_UNROLL
-#define NB200_MACH_UNROLL 1
-#endif
-#if NB200_MACH_UNROLL
-#define NB_MACH_FOR(i, MAXM, m) _Pragma("unroll") for (int i = 0; i < (MAXM); ++i)
-#define NB_MACH_IF(i, m) if ((i) < (m))
-#else
-#define NB_MACH_FOR(i, MAXM, m) for (int i = 0; i < (m); ++i)
-#define NB_MACH_IF(i, m)
-#endif
+// MAXM bounds m at compile time: the index-order sums over the multipliers are unrolled to MAXM trips with a predicate
+// i < m, so that their shuffles are issued back to back instead of one per loop trip (they sit on the serial path of
+// every generation).
 template <int MAXM>
 struct WarpDualMachine {
     double y, g, sigma, ycur, yprev, yprevprev, lo, hi;          // lane i: element i (lanes >= m: sigma = 0)
@@ -1423,9 +1310,10 @@ struct WarpDualMachine {
     {
         const double d = fabs(subx(ycur, yprev)), a = fabs(ycur);
         double dn = 0.0, xn = 0.0;
-        NB_MACH_FOR(i, MAXM, m) {
+#pragma unroll
+        for (int i = 0; i < MAXM; ++i) {
             const double di = __shfl_sync(0xffffffffu, d, i), ai = __shfl_sync(0xffffffffu, a, i);
-            NB_MACH_IF(i, m) { dn = addx(dn, di); xn = addx(xn, ai); }
+            if (i < m) { dn = addx(dn, di); xn = addx(xn, ai); }
         }
         if (dn < mulx(st.xtol_rel, xn)) return true;
         return !__any_sync(0xffffffffu, lane < m && d >= st.xtol_abs);
@@ -1505,10 +1393,11 @@ struct WarpDualMachine {
             wt = mulx(mulx(0.5, dy2), dinv);
         }
         double gs = fbase, ws = 0.0;                      // mma.c:123-125: the terms added in index order
-        NB_MACH_FOR(i, MAXM, m) {
+#pragma unroll
+        for (int i = 0; i < MAXM; ++i) {
             const double gi = __shfl_sync(0xffffffffu, gt, i), wi = __shfl_sync(0xffffffffu, wt, i);
             const int hi_ = __shfl_sync(0xffffffffu, (int) has, i);
-            NB_MACH_IF(i, m) if (hi_) { gs = addx(gs, gi); ws = addx(ws, wi); }
+            if (i < m) if (hi_) { gs = addx(gs, gi); ws = addx(ws, wi); }
         }
         gval = gs;
         wval = ws;
@@ -1583,9 +1472,10 @@ __device__ __noinline__ void solve_folder(const SolveArgs &sa, double *s_vs, dou
             }
         } else {
             double u = a.rho;
-            NB_MACH_FOR(i, MAXM, a.m) {
+#pragma unroll
+            for (int i = 0; i < MAXM; ++i) {
                 const double yi = __shfl_sync(0xffffffffu, mach.y, i);
-                NB_MACH_IF(i, a.m) u = addx(u, mulx(a.rhoc[i], yi));
+                if (i < a.m) u = addx(u, mulx(a.rhoc[i], yi));
             }
             NB_TR(if (lane == 0) sa.trace[16] = nb_globaltimer();)
             if (lane < a.m) slot_put(st->pub + 2 * lane, mach.y, sa.tag0 | 1ull);
@@ -1628,9 +1518,10 @@ __device__ __noinline__ void solve_folder(const SolveArgs &sa, double *s_vs, dou
                 const double gsum = __shfl_sync(0xffffffffu, total, (lane + 3) & 31);      // lane i < m: sum 3 + i
                 const double grad = lane < a.m ? -addx(cv, gsum) : 0.0;                     // -g_i(y)
                 double val = sa.fval;
-                NB_MACH_FOR(i, MAXM, a.m) {
+#pragma unroll
+                for (int i = 0; i < MAXM; ++i) {
                     const double yi = __shfl_sync(0xffffffffu, yt, i), ci = __shfl_sync(0xffffffffu, cv, i);
-                    NB_MACH_IF(i, a.m) val = addx(val, mulx(yi, ci));
+                    if (i < a.m) val = addx(val, mulx(yi, ci));
                 }
                 val = addx(val, __shfl_sync(0xffffffffu, total, 0));
                 finished = timed_out ? 1 : (mach.feed_pre(-val, grad, time_up != 0, lane) ? 1 : 0);
@@ -1661,9 +1552,10 @@ __device__ __noinline__ void solve_folder(const SolveArgs &sa, double *s_vs, dou
                 const double trial = next_final ? mach.y : mach.ycur;
                 const unsigned long long ntag = sa.tag0 | (gen + 1);
                 double u = a.rho;
-                NB_MACH_FOR(i, MAXM, a.m) {
+#pragma unroll
+                for (int i = 0; i < MAXM; ++i) {
                     const double ti = __shfl_sync(0xffffffffu, trial, i);
-                    NB_MACH_IF(i, a.m) u = addx(u, mulx(a.rhoc[i], ti));
+                    if (i < a.m) u = addx(u, mulx(a.rhoc[i], ti));
                 }
                 NB_TR(if (lane == 0 && gen + 1 < kTraceGens) sa.trace[16 * (gen + 1)] = nb_globaltimer();)
                 if (lane < a.m) slot_put(st->pub + 2 * lane, trial, ntag);
@@ -1680,7 +1572,7 @@ __device__ __noinline__ void solve_folder(const SolveArgs &sa, double *s_vs, dou
     }
 }
 
-template <int VARIANT, int MAXM, bool FULL, bool POL, int BLOCK, int UNROLL, int MINB, bool SB>
+template <int VARIANT, int MAXM, bool FULL, bool POL, int BLOCK, int MINB, bool SB>
 __global__ void __launch_bounds__(BLOCK, MINB) dual_solve_kernel(const __grid_constant__ SolveArgs sa)
 {
     constexpr int MR = MAXM > 0 ? MAXM : 1;
@@ -1720,18 +1612,14 @@ __global__ void __launch_bounds__(BLOCK, MINB) dual_solve_kernel(const __grid_co
         const unsigned long long c = s_claim[it & 1];
         const unsigned long long want = c / ngroups + 1;
         const unsigned gl = (unsigned) (c % ngroups);
-#if NB200_PRELOAD
         // the first chunk's operands are requested before anything else: they do not depend on the multipliers
         unsigned long long p_lo, p_hi;
         group_pairs(a.nchunks, a.nseg_total, a.chunk0, a.seg0 + gl, &p_lo, &p_hi);
         const unsigned long long p_first = p_lo + sub * 32 + lane;
         ChunkOperands<MAXM> first;
         load_chunk<MAXM, FULL, POL, SB>(a, a.m, pol, p_first, p_first < p_hi, first);
-#endif
         // wait until generation `want` is published (or the solve has finished); refresh the multipliers
         if (want != my_gen) {
-            // ... with the head of the group on its way from HBM to the L2 meanwhile
-            if (threadIdx.x == 32 && a.prefetch_chunks) prefetch_group_head<SB>(a, gl, a.prefetch_chunks);
             if (sub == 0) {                   // warp 0 polls, warp-uniformly: lane i < m: y_i, lane m: u, the others: flags
                 const int slot = lane < a.m ? lane : (lane == a.m ? kMaxParamM : kMaxParamM + 1);
                 const unsigned long long tag = sa.tag0 | want;
@@ -1756,14 +1644,6 @@ __global__ void __launch_bounds__(BLOCK, MINB) dual_solve_kernel(const __grid_co
             NB_TR(if (threadIdx.x == 0 && want < kTraceGens) { const unsigned long long t = nb_globaltimer();
                       atomicMax(&sa.trace[16 * want + 1], ~t); atomicMax(&sa.trace[16 * want + 2], t); })
             my_gen = want;
-            // Skew experiment (knob b200_stagger_ns, default 0).  The 6 warps that share an SM sub-partition (2 per CTA, 3
-            // CTAs) receive the multipliers at the same moment and, under round-robin issue, finish every chunk together,
-            // request the next one together and leave the fp64 pipe idle for a load latency per chunk.  A one-time offset
-            // of slot x stagger_ns at the start of a generation lets them take turns instead.
-            if (a.stagger_ns) {
-                const unsigned slot = (blockIdx.x / (a.sm_count ? a.sm_count : 1u)) * 2u + (unsigned) (sub >> 2);
-                if (slot) __nanosleep(slot * a.stagger_ns);
-            }
         }
         // claim the next group now; the result is parked in a register until the sweep is over
         if (threadIdx.x == 0) next_c = atomicAdd(&st->claim, 1ull);
@@ -1776,12 +1656,8 @@ __global__ void __launch_bounds__(BLOCK, MINB) dual_solve_kernel(const __grid_co
 #pragma unroll
         for (int k = 0; k < NV; ++k) acc[k] = 0.0;
         NB_TR(const unsigned long long tr_s0 = nb_globaltimer();)
-#if NB200_PRELOAD
         // (the 128-register instantiations, MINB <= 2, have room for the MMA pair form with 4 rows)
         sweep_group_preloaded<VARIANT, MAXM, FULL, POL, kPairMMA<MAXM> || (MINB <= 2 && MAXM <= 4), SB>(a, mu, pol, s_store != 0, p_first, p_hi, first, acc);
-#else
-        sweep_group<VARIANT, MAXM, FULL, UNROLL, POL, SB>(a, mu, pol, s_store != 0, gl, sub, lane, acc);
-#endif
 
         warp_fold<NV>(acc);
         double *srec = s_rec[parity];
@@ -1935,9 +1811,7 @@ __global__ void __launch_bounds__(kBlock, MINB) dual_solve_async_kernel(const __
         mu.active = a.active; mu.m = a.m;
         DivBy U;
         U.b = 1.0; U.r = 1.0; U.hb = 0x3ff00000; U.zero_ok = 1u;
-#if NB200_PAIR
         if (VARIANT != 0) U = prep_div(mu.u());
-#endif
         const bool store = s_store != 0;
         double acc[NV];
 #pragma unroll

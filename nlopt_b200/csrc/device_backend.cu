@@ -1134,13 +1134,7 @@ void DeviceBackend::fill_dual_args(DualArgs &a, const double *y, const DualScala
         // the mailbox holds records of <= 19 sums: the wide kernel exchanges through ncclAllGather
         for (int r = 0; r < 8; ++r) a.box[r] = (cm.active() && cm.use_p2p() && !wide && r < cm.world) ? cm.box_peer[r] : nullptr;
     }
-    a.l2_keep = l2_keep_mask() | (l1_prefetch_ ? kL1PrefetchBit : 0u);
-    // The L2 prefetch of a waiting sweeper is opt-in (knob b200_prefetch_chunks).  On the H100 (CCSAQ, m = 4) it made
-    // every size whose operands exceed the 50 MB L2 slower: 40.4 vs 33.2 us per evaluation at n = 8e5, 55.7 vs 48.3 at
-    // 1.25e6, 315 vs 307.5 at 1e7; it gained 5 % only at n = 4e5, where the operands stay in the L2.
-    a.prefetch_chunks = prefetch_forced_ ? prefetch_chunks_ : 0u;
-    a.stagger_ns = stagger_ns_;
-    a.sm_count = (unsigned) sm_count_;
+    a.l2_keep = l2_keep_mask();
     a.m = (int) m_;
     a.rho = sc.rho;
     a.half_rho = 0.5 * sc.rho;
@@ -1282,17 +1276,17 @@ template <int VARIANT, bool FULL, bool POL, bool SB>
 SolveKernel pick_solve_kernel(int maxm, bool roomy)
 {
     if (roomy) switch (maxm) {
-        case 1: return dual_solve_kernel<VARIANT, 1, FULL, POL, 256, 1, 2, SB>;
-        case 2: return dual_solve_kernel<VARIANT, 2, FULL, POL, 256, 1, 2, SB>;
-        case 4: return dual_solve_kernel<VARIANT, 4, FULL, POL, 256, 1, 2, SB>;
+        case 1: return dual_solve_kernel<VARIANT, 1, FULL, POL, 256, 2, SB>;
+        case 2: return dual_solve_kernel<VARIANT, 2, FULL, POL, 256, 2, SB>;
+        case 4: return dual_solve_kernel<VARIANT, 4, FULL, POL, 256, 2, SB>;
         default: break;
         }
     switch (maxm) {
-    case 1: return dual_solve_kernel<VARIANT, 1, FULL, POL, 256, 1, NB200_SOLVE_MINB4, SB>;
-    case 2: return dual_solve_kernel<VARIANT, 2, FULL, POL, 256, 1, NB200_SOLVE_MINB4, SB>;
-    case 4: return dual_solve_kernel<VARIANT, 4, FULL, POL, 256, 1, NB200_SOLVE_MINB4, SB>;
-    case 8: return dual_solve_kernel<VARIANT, 8, FULL, POL, 256, 1, 2, SB>;
-    default: return dual_solve_kernel<VARIANT, 16, FULL, POL, 256, 1, 2, SB>;
+    case 1: return dual_solve_kernel<VARIANT, 1, FULL, POL, 256, NB200_SOLVE_MINB4, SB>;
+    case 2: return dual_solve_kernel<VARIANT, 2, FULL, POL, 256, NB200_SOLVE_MINB4, SB>;
+    case 4: return dual_solve_kernel<VARIANT, 4, FULL, POL, 256, NB200_SOLVE_MINB4, SB>;
+    case 8: return dual_solve_kernel<VARIANT, 8, FULL, POL, 256, 2, SB>;
+    default: return dual_solve_kernel<VARIANT, 16, FULL, POL, 256, 2, SB>;
     }
 }
 // TMA-staged form (full-m, 1 / 2 / 4 rows): {stages, bytes of dynamic shared memory}.  A stage is (5 + m) x 4 KB,
@@ -1741,9 +1735,6 @@ bool DeviceBackend::configure(const char *key, long long value)
     if (k == "solve_tma") { solve_tma_ = (int) value; return true; }
     if (k == "solve_async") { solve_async_ = (int) value; return true; }
     if (k == "solve_minb") { solve_minb_ = (int) value; return true; }
-    if (k == "stagger_ns") { stagger_ns_ = value < 0 ? 0u : (unsigned) value; return true; }
-    if (k == "l1_prefetch") { l1_prefetch_ = value != 0; return true; }
-    if (k == "prefetch_chunks") { prefetch_chunks_ = value < 0 ? 0u : (unsigned) value; prefetch_forced_ = true; return true; }
     if (k == "l2_keep_mb") {
         l2_keep_bytes_ = value <= 0 ? 0 : (size_t) value << 20;
         // evict_last lines are only protected inside the persisting carve-out of the L2: size it to the request

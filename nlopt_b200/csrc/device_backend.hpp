@@ -1,13 +1,6 @@
 // device_backend.hpp -- HBM-resident state + kernel launches of the MMA/CCSAQ path.
 #pragma once
 
-#ifndef NB200_STAGGER_NS_DEFAULT
-#define NB200_STAGGER_NS_DEFAULT 0
-#endif
-#ifndef NB200_SOLVE_ASYNC_DEFAULT
-#define NB200_SOLVE_ASYNC_DEFAULT 0
-#endif
-
 #include <cuda_runtime.h>
 
 #include <string>
@@ -122,12 +115,8 @@ private:
     std::vector<double> wide_host_;
     size_t l2_keep_bytes_ = 0;        // operand bytes to load evict_last (knob b200_l2_keep_mb)
     int solve_tma_ = -1;              // knob b200_solve_tma: -1 by rows, bounds and size (DeviceBackend::dual_solve), 0 register form, 1 TMA-staged form
-    int solve_async_ = NB200_SOLVE_ASYNC_DEFAULT;   // knob b200_solve_async: 0 register form, 2 / 3: per-thread cp.async operand ring of 2 / 3 stages
+    int solve_async_ = 0;             // knob b200_solve_async: 0 register form, 2 / 3: per-thread cp.async operand ring of 2 / 3 stages
     int solve_minb_ = 0;              // knob b200_solve_minb: 0 by size, 2 / 3: force the 2- / 3-CTAs-per-SM instantiation of the solve kernel
-    unsigned stagger_ns_ = NB200_STAGGER_NS_DEFAULT;   // knob b200_stagger_ns: start-of-generation skew between warps sharing an SM sub-partition
-    bool l1_prefetch_ = false;        // knob b200_l1_prefetch (experiment): L1 prefetch of the next chunk inside the sweep
-    bool prefetch_forced_ = false;
-    unsigned prefetch_chunks_ = 3;    // knob b200_prefetch_chunks (solve kernel: L2 prefetch of a waiting sweeper's next group)
     size_t out_rec_ = 0;              // doubles per result record (>= 24, >= 3 + m)
     unsigned long long solve_launch_id_ = 0;   // tag = launch id << 40 | generation: never matches a stale slot
     bool fused_solve_ok_ = true;

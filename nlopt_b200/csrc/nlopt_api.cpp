@@ -1100,11 +1100,8 @@ nlopt_result run_ccsa(nlopt_opt opt, double *x_host, double *x_dev, double *minf
     if (nlopt_has_param(opt, "b200_kernel_cfg")) be->configure("kernel_cfg", (long long) nlopt_get_param(opt, "b200_kernel_cfg", 0.0));
     if (nlopt_has_param(opt, "b200_ctas_per_sm")) be->configure("ctas_per_sm", (long long) nlopt_get_param(opt, "b200_ctas_per_sm", 0.0));
     if (nlopt_has_param(opt, "b200_solve_tma")) be->configure("solve_tma", (long long) nlopt_get_param(opt, "b200_solve_tma", -1.0));
-    if (nlopt_has_param(opt, "b200_stagger_ns")) be->configure("stagger_ns", (long long) nlopt_get_param(opt, "b200_stagger_ns", 0.0));
     if (nlopt_has_param(opt, "b200_solve_minb")) be->configure("solve_minb", (long long) nlopt_get_param(opt, "b200_solve_minb", 0.0));
     if (nlopt_has_param(opt, "b200_solve_async")) be->configure("solve_async", (long long) nlopt_get_param(opt, "b200_solve_async", 0.0));
-    if (nlopt_has_param(opt, "b200_l1_prefetch")) be->configure("l1_prefetch", (long long) nlopt_get_param(opt, "b200_l1_prefetch", 0.0));
-    if (nlopt_has_param(opt, "b200_prefetch_chunks")) be->configure("prefetch_chunks", (long long) nlopt_get_param(opt, "b200_prefetch_chunks", 0.0));
     if (nlopt_has_param(opt, "b200_l2_keep_mb")) be->configure("l2_keep_mb", (long long) nlopt_get_param(opt, "b200_l2_keep_mb", 0.0));
 
     nb200::StopCriteria st;                          /* optimize.c:553-566 */

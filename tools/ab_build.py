@@ -1,10 +1,10 @@
 """A/B builds of the library: the same sources with extra -D switches, written to build/ab/NAME/ (libnlopt_b200.so +
 libnlopt_b200_problems.so).  A run picks one with NLOPT_B200_LIBDIR=build/ab/NAME (nlopt_b200/_capi.py), so one GPU
 session can time several compile-time variants back to back -- no template explosion in the product build.
-    python tools/ab_build.py NAME [-DNB200_PAIR=0 ...]        # no GPU needed
-Switches in use: NB200_PAIR (ccsa_kernels.cuh: pair_math.cuh closed forms, default 1), NB200_SOLVE_MINB4 (min CTAs/SM of
-the solve kernel with <= 4 gradient rows, default 3), NB200_SOLVE_TMA_IDX_STAGES4 (stages of the sigma-index TMA solve kernel
-with 4 rows, default 3), NB200_SIGMA_PALETTE_CAP (entries of the sigma palette, default 65535)."""
+    python tools/ab_build.py NAME [-DNB200_SOLVE_MINB4=2 ...]        # no GPU needed
+Switches in use: NB200_SOLVE_MINB4 (min CTAs/SM of the solve kernel with <= 4 gradient rows, default 3),
+NB200_SOLVE_TMA_IDX_STAGES4 (stages of the sigma-index TMA solve kernel with 4 rows, default 3), NB200_SIGMA_PALETTE_CAP
+(entries of the sigma palette, default 65535)."""
 import os
 import sys
 
