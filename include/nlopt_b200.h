@@ -27,6 +27,12 @@
  * and sharded entry points, under LD_MMA, LD_CCSAQ and the AUGLAG family
  * (sharded objectives under LD_MMA / LD_CCSAQ only).
  *
+ * Box bounds may live in GPU memory too: nlopt_b200_set_lower_bounds_device /
+ * nlopt_b200_set_upper_bounds_device copy n doubles from a device array,
+ * snap them as the host setters do, and put the object in device mode (one
+ * GPU), where a run checks the start point and detects uniform bounds on the
+ * device.
+ *
  * The `nlopt_b200_*` symbols are additive extensions (device-resident
  * callbacks, kernel-level access to the dual evaluation, multi-GPU sharding,
  * statistics).  No torch / CUDA types appear in any signature: device
@@ -376,6 +382,20 @@ nlopt_result nlopt_b200_set_max_objective_sharded(nlopt_opt opt, nlopt_b200_sfun
 nlopt_result nlopt_b200_add_inequality_constraint_sharded(nlopt_opt opt, nlopt_b200_sfunc fc, void *fc_data, double tol);
 /* like nlopt_optimize, but x_dev is a device array of this rank's shard (in/out) */
 nlopt_result nlopt_b200_optimize_device(nlopt_opt opt, double *x_dev, double *opt_f);
+/* Box bounds from device memory.  The call copies the n doubles at lb_dev / ub_dev into device memory the object owns
+ * (on the current device) and returns when the copy is complete, so the buffer may be reused at once; the work that
+ * produces it must be complete before the call, as for nlopt_b200_optimize_device.  The copy is snapped on the device
+ * as nlopt_set_lower_bounds / nlopt_set_upper_bounds snap (a subnormally thin interval is shut), giving the same bits.
+ * The first such call puts the object in device mode for both arrays (the other one is uploaded once); a run then
+ * copies them device to device, checks the start point on the device (NLOPT_INVALID_ARGS and the reference's
+ * "bounds %d fail" message, no evaluation) and reads each array as one scalar where all its lanes have the bits of
+ * lane 0.  Any host bound setter downloads both arrays and leaves device mode; nlopt_get_*_bounds,
+ * nlopt_set_local_optimizer and the initial-step heuristics read the device values; nlopt_copy duplicates them.
+ * NULL: NLOPT_INVALID_ARGS; n == 0: no-op; no usable device: NLOPT_FAILURE, bounds unchanged; several ranks, a run on
+ * another current device, or preconditioned CCSAQ: NLOPT_INVALID_ARGS.  The deprecated nlopt_minimize* API takes host
+ * bounds only. */
+nlopt_result nlopt_b200_set_lower_bounds_device(nlopt_opt opt, const double *lb_dev);
+nlopt_result nlopt_b200_set_upper_bounds_device(nlopt_opt opt, const double *ub_dev);
 
 /* Run statistics of the last nlopt_optimize on this object; after an NLOPT_AUGLAG* run, those of its last
  * sub-optimisation. */

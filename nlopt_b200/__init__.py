@@ -59,6 +59,22 @@ def _ptr(a):
     return a.ctypes.data_as(c_double_p)
 
 
+def _cuda_f64(v, n):
+    """the device pointer of `v`, an object with __cuda_array_interface__ describing n contiguous float64 values"""
+    cai = v.__cuda_array_interface__
+    shape, strides = tuple(cai["shape"]), cai.get("strides")
+    contiguous = []
+    step = 8
+    for d in reversed(shape):
+        contiguous.insert(0, step)
+        step *= d
+    if (cai["typestr"] != "<f8" or int(np.prod(shape, dtype=np.int64)) != n
+            or (strides is not None and tuple(strides) != tuple(contiguous))):
+        raise ValueError(f"device bounds need a contiguous float64 CUDA array of {n} values (got typestr "
+                         f"{cai['typestr']}, shape {shape}, strides {strides})")
+    return cai["data"][0]
+
+
 class _DeviceArray:
     """float64 device memory of the library, handed to torch.as_tensor as a zero-copy view (no stream: the view is
     used on the library stream itself)"""
@@ -515,11 +531,30 @@ class opt:
         self._check(fn(self._h, _ptr(a)))
         return a
 
+    # bounds: a scalar, a host array, or a device array (__cuda_array_interface__: a CUDA tensor, a CuPy array ...), which
+    # the library copies into its own device memory (nlopt_b200_set_*_bounds_device); a torch tensor's current stream is
+    # synchronised first
+    def _set_bounds(self, vec_fn, scalar_fn, dev_name, v):
+        if not hasattr(v, "__cuda_array_interface__"):
+            self._set_vec_or_scalar(vec_fn, scalar_fn, v)
+            return
+        ptr = _cuda_f64(v, self._n)
+        dev_fn = getattr(self._lib, dev_name)
+        if type(v).__module__.split(".")[0] != "torch":
+            self._check(dev_fn(self._h, ptr))
+            return
+        import torch
+        with torch.cuda.device(v.device):          # the object's arrays go to the tensor's device
+            torch.cuda.current_stream().synchronize()
+            self._check(dev_fn(self._h, ptr))
+
     def set_lower_bounds(self, v):
-        self._set_vec_or_scalar(self._lib.nlopt_set_lower_bounds, self._lib.nlopt_set_lower_bounds1, v)
+        self._set_bounds(self._lib.nlopt_set_lower_bounds, self._lib.nlopt_set_lower_bounds1,
+                         "nlopt_b200_set_lower_bounds_device", v)
 
     def set_upper_bounds(self, v):
-        self._set_vec_or_scalar(self._lib.nlopt_set_upper_bounds, self._lib.nlopt_set_upper_bounds1, v)
+        self._set_bounds(self._lib.nlopt_set_upper_bounds, self._lib.nlopt_set_upper_bounds1,
+                         "nlopt_b200_set_upper_bounds_device", v)
 
     def set_lower_bound(self, i, v):
         self._check(self._lib.nlopt_set_lower_bound(self._h, int(i), float(v)))

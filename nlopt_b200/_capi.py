@@ -196,6 +196,8 @@ _EXT = {
     "nlopt_b200_set_min_objective_sharded": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "nlopt_b200_add_inequality_constraint_sharded": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_double]),
     "nlopt_b200_optimize_device": (C.c_int, [C.c_void_p, C.c_void_p, c_double_p]),
+    "nlopt_b200_set_lower_bounds_device": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "nlopt_b200_set_upper_bounds_device": (C.c_int, [C.c_void_p, C.c_void_p]),
     "nlopt_b200_get_stats": (C.c_int, [C.c_void_p, C.POINTER(Stats)]),
     "nlopt_b200_dual_create": (C.c_void_p, [C.c_int, C.c_uint, C.c_uint]),
     "nlopt_b200_dual_destroy": (None, [C.c_void_p]),

@@ -47,6 +47,12 @@ struct PenaltySpec {
     const int *force_stop = nullptr;         // the outer object's force-stop flag (auglag.c:39)
 };
 
+// The start-point test of optimize.c:547-551 run on the device: the smallest failing index and its three values.
+struct StartCheck {
+    long long bad = -1;          // -1: every lb <= x <= ub
+    double lb = 0, x = 0, ub = 0;
+};
+
 struct BackendConfig {
     Variant variant = kMMA;
     unsigned n = 0;                          // global problem size
@@ -55,6 +61,11 @@ struct BackendConfig {
     std::vector<FuncSpec> constraints;       // inequality constraint objects, in registration order
     const double *lb = nullptr, *ub = nullptr;   // host, n entries
     bool lb_uniform = false, ub_uniform = false; // all entries equal lb[0] / ub[0]: fill on the device, no H2D
+    // ... or device bounds (an object in device mode, one rank): copied D2D, checked against the start point on the
+    // device, and read as two scalars where each array is bitwise uniform.  A failed check is reported in *start_check
+    // and the set-up still succeeds; the caller ends the run.
+    const double *lb_dev = nullptr, *ub_dev = nullptr;
+    StartCheck *start_check = nullptr;
     const double *x0_host = nullptr;         // host start point (n entries) ...
     double *x_dev = nullptr;                 // ... or this rank's device shard (device mode, in/out)
     const double *sigma_init = nullptr;      // nlopt initial step (host) or null
@@ -65,5 +76,23 @@ struct BackendConfig {
 };
 
 Backend *make_backend(const BackendConfig &cfg, std::string *err);
+
+// The bounds of an nlopt_opt in device mode (nlopt_b200_set_*_bounds_device, implemented in device_backend.cu): n
+// doubles each, on the device that was current at the first device setter.  The API layer reaches them through this
+// interface only, so nlopt_api.cpp references no CUDA code (the host-logic tests link it without device_backend.cu).
+// Methods return false with a message in *err.
+class DeviceBounds {
+public:
+    virtual ~DeviceBounds() {}
+    virtual const double *lb() const = 0;
+    virtual const double *ub() const = 0;
+    virtual bool download(double *lb_host, double *ub_host, std::string *err) const = 0;
+    // *dst (allocated on this object's device when null) <- these values, device to device
+    virtual bool copy_into(DeviceBounds **dst, std::string *err) const = 0;
+    // a run may use them: one rank, and their device is the current one
+    virtual bool runs_here(std::string *err) const = 0;
+    // the start-point test against these bounds, for a start point in host memory or on the device (one of them)
+    virtual bool check(const double *x_host, const double *x_dev, StartCheck *out, std::string *err) const = 0;
+};
 
 }  // namespace nb200

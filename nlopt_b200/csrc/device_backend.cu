@@ -9,12 +9,16 @@
 #include <cstdlib>
 #include <cstring>
 #include <map>
+#include <memory>
 #include <mutex>
+#include <string>
 #include <vector>
 
+#include "bounds_kernels.cuh"
 #include "ccsa_kernels.cuh"
 #include "comm.hpp"
 #include "dual_mma.hpp"
+#include "nlopt_object.hpp"
 #include "synth.cuh"
 #include "terms_kernels.cuh"
 
@@ -184,6 +188,32 @@ constexpr size_t kGuard = 8;        // doubles of guard around x and xcur (halo 
 
 int pick_maxm(int m) { return m == 0 ? 0 : m <= 1 ? 1 : m <= 2 ? 2 : m <= 4 ? 4 : m <= 8 ? 8 : 16; }
 
+std::string no_device_message(cudaError_t e)
+{
+    return std::string("no usable CUDA device (") + cudaGetErrorString(e) +
+           "); libnlopt_b200 runs NLOPT_LD_MMA/NLOPT_LD_CCSAQ on the GPU only";
+}
+
+// bounds_check_kernel over n lanes and the copy of its report into pinned host memory, on stream s
+cudaError_t enqueue_bounds_check(const double *lb, const double *ub, const double *x, unsigned n, BoundsReport *rep_dev,
+                                 BoundsReport *rep_host, int sms, cudaStream_t s)
+{
+    cudaError_t e = cudaMemsetAsync(rep_dev, 0, sizeof(BoundsReport), s);
+    if (e == cudaSuccess) e = cudaMemsetAsync(&rep_dev->first_bad, 0xff, sizeof(unsigned), s);
+    if (e != cudaSuccess) return e;
+    bounds_check_kernel<<<grid_for(n, sms), kBlock, 0, s>>>(lb, ub, x, n, rep_dev);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    return cudaMemcpyAsync(rep_host, rep_dev, sizeof(BoundsReport), cudaMemcpyDeviceToHost, s);
+}
+
+void read_bounds_report(const BoundsReport &r, StartCheck *out)
+{
+    out->bad = r.first_bad == 0xffffffffu ? -1 : (long long) r.first_bad;
+    out->lb = r.lb;
+    out->x = r.x;
+    out->ub = r.ub;
+}
+
 }  // namespace
 
 DeviceBackend::DeviceBackend() {}
@@ -254,9 +284,7 @@ bool DeviceBackend::alloc_state()
 {
     int ndev = 0;
     cudaError_t e = cudaGetDeviceCount(&ndev);
-    if (e != cudaSuccess || ndev == 0)
-        return fail(std::string("no usable CUDA device (") + cudaGetErrorString(e) +
-                    "); libnlopt_b200 runs NLOPT_LD_MMA/NLOPT_LD_CCSAQ on the GPU only");
+    if (e != cudaSuccess || ndev == 0) return fail(no_device_message(e));
     Comm &comm = Comm::instance();
     if (comm.active()) {
         device_ = comm.device;
@@ -434,32 +462,30 @@ bool DeviceBackend::setup(const BackendConfig &cfg)
         NB_CUDA(cudaMemsetAsync(pen_rows_, 0, (size_t) pen_total_ * geo_.ld * sizeof(double), stream_));
     }
     // bounds and start point
-    if (cfg.lb_uniform) {
-        fill_kernel<<<grid_for(nl, sm_count_), kBlock, 0, stream_>>>(lb_, cfg.lb[0], nl);
-        ++stats_->kernel_launches;
+    if (cfg.lb_dev) {                         // device bounds: uniformity is known after the check below
+        if (Comm::instance().active()) return fail("device bounds run on one rank");
+        NB_CUDA(cudaMemcpyAsync(lb_, cfg.lb_dev, nl * sizeof(double), cudaMemcpyDeviceToDevice, stream_));
+        NB_CUDA(cudaMemcpyAsync(ub_, cfg.ub_dev, nl * sizeof(double), cudaMemcpyDeviceToDevice, stream_));
     } else {
-        NB_CUDA(cudaMemcpyAsync(lb_, cfg.lb + j0, nl * sizeof(double), cudaMemcpyHostToDevice, stream_));
-        stats_->h2d_bytes += nl * sizeof(double);
+        if (cfg.lb_uniform) {
+            fill_kernel<<<grid_for(nl, sm_count_), kBlock, 0, stream_>>>(lb_, cfg.lb[0], nl);
+            ++stats_->kernel_launches;
+        } else {
+            NB_CUDA(cudaMemcpyAsync(lb_, cfg.lb + j0, nl * sizeof(double), cudaMemcpyHostToDevice, stream_));
+            stats_->h2d_bytes += nl * sizeof(double);
+        }
+        if (cfg.ub_uniform) {
+            fill_kernel<<<grid_for(nl, sm_count_), kBlock, 0, stream_>>>(ub_, cfg.ub[0], nl);
+            ++stats_->kernel_launches;
+        } else {
+            NB_CUDA(cudaMemcpyAsync(ub_, cfg.ub + j0, nl * sizeof(double), cudaMemcpyHostToDevice, stream_));
+            stats_->h2d_bytes += nl * sizeof(double);
+        }
+        scalar_bounds_ = cfg.lb_uniform && cfg.ub_uniform;
+        lb_u_ = scalar_bounds_ ? cfg.lb[0] : 0.0;
+        ub_u_ = scalar_bounds_ ? cfg.ub[0] : 0.0;
     }
-    if (cfg.ub_uniform) {
-        fill_kernel<<<grid_for(nl, sm_count_), kBlock, 0, stream_>>>(ub_, cfg.ub[0], nl);
-        ++stats_->kernel_launches;
-    } else {
-        NB_CUDA(cudaMemcpyAsync(ub_, cfg.ub + j0, nl * sizeof(double), cudaMemcpyHostToDevice, stream_));
-        stats_->h2d_bytes += nl * sizeof(double);
-    }
-    scalar_bounds_ = cfg.lb_uniform && cfg.ub_uniform;
-    lb_u_ = scalar_bounds_ ? cfg.lb[0] : 0.0;
-    ub_u_ = scalar_bounds_ ? cfg.ub[0] : 0.0;
     sidx_valid_ = false;
-    if (scalar_bounds_ && m_ == 4) {          // the sigma index and its palette (device + pinned staging), sized for the cap once
-        if (!small_dev((void **) &sidx_, geo_.ld * sizeof(unsigned short))) return false;
-        if (!small_dev((void **) &pal_, SigmaPalette::kCap * sizeof(double))) return false;
-        if (!small_dev((void **) &next_, SigmaPalette::kCap * 3 * sizeof(unsigned short))) return false;
-        if (!small_pinned((void **) &pal_pinned_, SigmaPalette::kCap * sizeof(double))) return false;
-        if (!small_pinned((void **) &next_pinned_, SigmaPalette::kCap * 3 * sizeof(unsigned short))) return false;
-        NB_CUDA(cudaMemsetAsync(sidx_, 0, geo_.ld * sizeof(unsigned short), stream_));
-    }
     bool any_host_cb = cfg.objective.f != nullptr;
     for (const FuncSpec &c : cfg.constraints) any_host_cb = any_host_cb || c.f || c.mf;
     if (cfg.penalty)
@@ -496,8 +522,30 @@ bool DeviceBackend::setup(const BackendConfig &cfg)
         NB_CUDA(cudaMemcpyAsync(x_, cfg.x_dev, nl * sizeof(double), cudaMemcpyDeviceToDevice, stream_));
     } else
         return fail("no start point");
+    BoundsReport *rep_host = nullptr;
+    if (cfg.lb_dev) {                         // before any callback; read back with the synchronisation below
+        BoundsReport *rep_dev = nullptr;
+        if (!small_dev((void **) &rep_dev, sizeof(BoundsReport))) return false;
+        if (!small_pinned((void **) &rep_host, sizeof(BoundsReport))) return false;
+        NB_CUDA(enqueue_bounds_check(lb_, ub_, x_, (unsigned) nl, rep_dev, rep_host, sm_count_, stream_));
+        ++stats_->kernel_launches;
+    }
     if (!set_norm_arrays(cfg.x_weights, cfg.xtol_abs)) return false;
     NB_CUDA(cudaStreamSynchronize(stream_));
+    if (rep_host) {
+        if (cfg.start_check) read_bounds_report(*rep_host, cfg.start_check);
+        scalar_bounds_ = rep_host->nonuniform == 0;
+        lb_u_ = scalar_bounds_ ? rep_host->lb0 : 0.0;
+        ub_u_ = scalar_bounds_ ? rep_host->ub0 : 0.0;
+    }
+    if (scalar_bounds_ && m_ == 4) {          // the sigma index and its palette (device + pinned staging), sized for the cap once
+        if (!small_dev((void **) &sidx_, geo_.ld * sizeof(unsigned short))) return false;
+        if (!small_dev((void **) &pal_, SigmaPalette::kCap * sizeof(double))) return false;
+        if (!small_dev((void **) &next_, SigmaPalette::kCap * 3 * sizeof(unsigned short))) return false;
+        if (!small_pinned((void **) &pal_pinned_, SigmaPalette::kCap * sizeof(double))) return false;
+        if (!small_pinned((void **) &next_pinned_, SigmaPalette::kCap * 3 * sizeof(unsigned short))) return false;
+        NB_CUDA(cudaMemsetAsync(sidx_, 0, geo_.ld * sizeof(unsigned short), stream_));
+    }
     cand_in_x_ = true;                       // xcur == x at the start (mma.c:220)
     return true;
 }
@@ -1787,6 +1835,147 @@ long long DeviceBackend::query(const char *key) const
 
 void release_cached_blocks() { BlockCache::get().clear(); }
 
+// ------------------------------------------------------------------------------------------------
+// bounds of an object in device mode.  The work goes to the per-thread default stream and is complete on return, so a
+// caller may reuse its buffers at once (NLopt's copy semantics).
+
+namespace {
+
+bool cuda_ok(cudaError_t e, const char *what, std::string *err)
+{
+    if (e == cudaSuccess) return true;
+    *err = std::string(what) + ": " + cudaGetErrorString(e);
+    return false;
+}
+
+// makes `device` current for the lifetime of the guard
+struct DeviceGuard {
+    int prev = -1;
+    explicit DeviceGuard(int device)
+    {
+        if (cudaGetDevice(&prev) != cudaSuccess || prev == device || cudaSetDevice(device) != cudaSuccess) prev = -1;
+    }
+    ~DeviceGuard()
+    {
+        if (prev >= 0) cudaSetDevice(prev);
+    }
+};
+
+class DeviceBoundsImpl : public DeviceBounds {
+public:
+    explicit DeviceBoundsImpl(unsigned n) : n_(n) {}
+    ~DeviceBoundsImpl() override
+    {
+        if (p_) {
+            DeviceGuard g(device_);
+            cudaFree(p_);
+        }
+    }
+    const double *lb() const override { return p_; }
+    const double *ub() const override { return p_ + n_; }
+
+    // both arrays on the current device
+    bool alloc(std::string *err)
+    {
+        int ndev = 0;
+        const cudaError_t e = cudaGetDeviceCount(&ndev);
+        if (e != cudaSuccess || ndev == 0) {
+            *err = no_device_message(e);
+            return false;
+        }
+        return cuda_ok(cudaGetDevice(&device_), "cudaGetDevice", err) &&
+               cuda_ok(cudaMalloc(&p_, 2 * bytes()), "cudaMalloc", err);
+    }
+    // lb / ub <- lb_src / ub_src (any memory CUDA can read; null: keep)
+    bool upload(const double *lb_src, const double *ub_src, std::string *err)
+    {
+        return (!lb_src || cuda_ok(cudaMemcpyAsync(p_, lb_src, bytes(), cudaMemcpyDefault, cudaStreamPerThread), "cudaMemcpyAsync", err)) &&
+               (!ub_src || cuda_ok(cudaMemcpyAsync(p_ + n_, ub_src, bytes(), cudaMemcpyDefault, cudaStreamPerThread), "cudaMemcpyAsync", err)) &&
+               cuda_ok(cudaStreamSynchronize(cudaStreamPerThread), "cudaStreamSynchronize", err);
+    }
+    // the caller's n doubles into the lower (or upper) array, then the setters' snap against the other one
+    bool set(bool lower, const double *src, std::string *err)
+    {
+        DeviceGuard g(device_);
+        double *dst = lower ? p_ : p_ + n_;
+        int sms = 0;
+        if (!cuda_ok(cudaMemcpyAsync(dst, src, bytes(), cudaMemcpyDefault, cudaStreamPerThread), "cudaMemcpyAsync", err) ||
+            !cuda_ok(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device_), "cudaDeviceGetAttribute", err))
+            return false;
+        snap_bounds_kernel<<<grid_for(n_, sms), kBlock, 0, cudaStreamPerThread>>>(dst, lower ? p_ + n_ : p_, lower, n_);
+        return cuda_ok(cudaGetLastError(), "snap_bounds_kernel", err) &&
+               cuda_ok(cudaStreamSynchronize(cudaStreamPerThread), "cudaStreamSynchronize", err);
+    }
+    bool download(double *lb_host, double *ub_host, std::string *err) const override
+    {
+        return cuda_ok(cudaMemcpyAsync(lb_host, p_, bytes(), cudaMemcpyDefault, cudaStreamPerThread), "cudaMemcpyAsync", err) &&
+               cuda_ok(cudaMemcpyAsync(ub_host, p_ + n_, bytes(), cudaMemcpyDefault, cudaStreamPerThread), "cudaMemcpyAsync", err) &&
+               cuda_ok(cudaStreamSynchronize(cudaStreamPerThread), "cudaStreamSynchronize", err);
+    }
+    bool copy_into(DeviceBounds **dst, std::string *err) const override
+    {
+        DeviceGuard g(device_);
+        if (!*dst) {
+            DeviceBoundsImpl *d = new DeviceBoundsImpl(n_);
+            if (!d->alloc(err)) {
+                delete d;
+                return false;
+            }
+            *dst = d;
+        }
+        DeviceBoundsImpl *d = static_cast<DeviceBoundsImpl *>(*dst);
+        return cuda_ok(cudaMemcpyAsync(d->p_, p_, 2 * bytes(), cudaMemcpyDefault, cudaStreamPerThread), "cudaMemcpyAsync", err) &&
+               cuda_ok(cudaStreamSynchronize(cudaStreamPerThread), "cudaStreamSynchronize", err);
+    }
+    bool runs_here(std::string *err) const override
+    {
+        if (Comm::instance().active()) {
+            *err = "device bounds (nlopt_b200_set_*_bounds_device) run on one rank in this library";
+            return false;
+        }
+        int d = -1;
+        cudaGetDevice(&d);
+        if (d != device_) {
+            *err = "the device bounds live on CUDA device " + std::to_string(device_) + " but device " + std::to_string(d) +
+                   " is current";
+            return false;
+        }
+        return true;
+    }
+    bool check(const double *x_host, const double *x_dev, StartCheck *out, std::string *err) const override
+    {
+        DeviceGuard g(device_);
+        const cudaStream_t s = cudaStreamPerThread;
+        BoundsReport *rep_dev = nullptr, *rep_host = nullptr;
+        double *x_stage = nullptr;
+        int sms = 0;
+        bool good = cuda_ok(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device_), "cudaDeviceGetAttribute", err) &&
+                    cuda_ok(cached_malloc((double **) &rep_dev, sizeof(BoundsReport)), "cudaMalloc", err) &&
+                    cuda_ok(cached_host_alloc((double **) &rep_host, sizeof(BoundsReport)), "cudaHostAlloc", err);
+        if (good && x_host) {
+            good = cuda_ok(cached_malloc(&x_stage, bytes()), "cudaMalloc", err) &&
+                   cuda_ok(cudaMemcpyAsync(x_stage, x_host, bytes(), cudaMemcpyHostToDevice, s), "cudaMemcpyAsync", err);
+            x_dev = x_stage;
+        }
+        good = good && cuda_ok(enqueue_bounds_check(lb(), ub(), x_dev, n_, rep_dev, rep_host, sms, s), "bounds_check_kernel", err) &&
+               cuda_ok(cudaStreamSynchronize(s), "cudaStreamSynchronize", err);
+        if (good) read_bounds_report(*rep_host, out);
+        cudaStreamSynchronize(s);
+        if (x_stage) BlockCache::get().give(false, bytes(), x_stage, device_);
+        if (rep_dev) BlockCache::get().give(false, sizeof(BoundsReport), rep_dev, device_);
+        if (rep_host) BlockCache::get().give(true, sizeof(BoundsReport), rep_host);
+        return good;
+    }
+
+private:
+    size_t bytes() const { return (size_t) n_ * sizeof(double); }
+    unsigned n_;
+    int device_ = -1;
+    double *p_ = nullptr;            // lb | ub
+};
+
+}  // namespace
+
 Backend *make_backend(const BackendConfig &cfg, std::string *err)
 {
     DeviceBackend *be = new DeviceBackend();
@@ -2011,6 +2200,41 @@ int nlopt_b200_device_count(void)
 }
 
 void nlopt_b200_release_cached_memory(void) { nb200::release_cached_blocks(); }
+
+/* device bounds (the rest of the bounds API is in nlopt_api.cpp).  An object whose first device setter fails keeps its
+   host bounds. */
+static nlopt_result set_bounds_device(nlopt_opt opt, const double *src, bool lower)
+{
+    if (!opt) return NLOPT_INVALID_ARGS;
+    opt->errmsg.clear();
+    opt->has_errmsg = false;
+    if (!src) return NLOPT_INVALID_ARGS;
+    if (opt->n == 0) return NLOPT_SUCCESS;
+    auto refuse = [opt](nlopt_result r, const std::string &msg) {
+        opt->errmsg = msg;
+        opt->has_errmsg = true;
+        return r;
+    };
+    if (nb200::Comm::instance().active())
+        return refuse(NLOPT_INVALID_ARGS, "device bounds (nlopt_b200_set_*_bounds_device) run on one rank in this library");
+    std::string err;
+    std::unique_ptr<nb200::DeviceBoundsImpl> fresh;
+    nb200::DeviceBoundsImpl *b = static_cast<nb200::DeviceBoundsImpl *>(opt->dbounds);
+    if (!b) {                                /* entering device mode: the other array goes up once */
+        fresh.reset(new nb200::DeviceBoundsImpl(opt->n));
+        if (!fresh->alloc(&err) || !fresh->upload(lower ? nullptr : opt->lb.data(), lower ? opt->ub.data() : nullptr, &err))
+            return refuse(NLOPT_FAILURE, err);
+        b = fresh.get();
+    }
+    if (!b->set(lower, src, &err)) return refuse(NLOPT_FAILURE, err);
+    if (fresh) opt->dbounds = fresh.release();
+    opt->lb_ub_mirror = false;
+    (lower ? opt->lb_uniform : opt->ub_uniform) = false;
+    return NLOPT_SUCCESS;
+}
+
+nlopt_result nlopt_b200_set_lower_bounds_device(nlopt_opt opt, const double *lb_dev) { return set_bounds_device(opt, lb_dev, true); }
+nlopt_result nlopt_b200_set_upper_bounds_device(nlopt_opt opt, const double *ub_dev) { return set_bounds_device(opt, ub_dev, false); }
 
 const char *nlopt_b200_build_info(void)
 {

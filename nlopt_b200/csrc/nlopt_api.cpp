@@ -60,6 +60,42 @@ void snap_upper(nlopt_opt o, unsigned i)
     if (o->lb[i] < o->ub[i] && is_tiny(o->ub[i] - o->lb[i])) o->ub[i] = o->lb[i];
 }
 
+// device mode: the bounds live in opt->dbounds (nlopt_b200_set_*_bounds_device)
+bool device_mode(const nlopt_opt o) { return o->dbounds != nullptr; }
+
+// Every host reader of the bounds goes through here: in device mode one download of both arrays into lb / ub, which
+// stay valid until a device setter changes the device arrays; false (with a message) when the download fails.
+bool host_bounds(nlopt_opt o)
+{
+    if (!device_mode(o) || o->lb_ub_mirror) return true;
+    std::string err;
+    if (!o->dbounds->download(o->lb.data(), o->ub.data(), &err)) {
+        set_err(o, "%s", err.c_str());
+        return false;
+    }
+    o->lb_ub_mirror = true;
+    return true;
+}
+
+// a host setter: the device values come down, and the object continues on host arrays
+bool leave_device_mode(nlopt_opt o)
+{
+    if (!host_bounds(o)) return false;
+    delete o->dbounds;
+    o->dbounds = nullptr;
+    o->lb_ub_mirror = false;
+    return true;
+}
+
+// a run in device mode: one rank, on the device that holds the arrays
+bool device_mode_runs_here(nlopt_opt o)
+{
+    std::string err;
+    if (o->dbounds->runs_here(&err)) return true;
+    set_err(o, "%s", err.c_str());
+    return false;
+}
+
 bool is_auglag(nlopt_algorithm a)
 {
     return a == NLOPT_AUGLAG || a == NLOPT_AUGLAG_EQ || a == NLOPT_LN_AUGLAG || a == NLOPT_LN_AUGLAG_EQ
@@ -255,6 +291,7 @@ void nlopt_destroy(nlopt_opt opt)
     }
     for (NamedParam *p : opt->params) delete p;
     nlopt_destroy(opt->local_opt);
+    delete opt->dbounds;
     delete opt;
 }
 
@@ -264,11 +301,18 @@ nlopt_opt nlopt_copy(const nlopt_opt opt)
     nlopt_opt c = new (std::nothrow) nlopt_opt_s(*opt);
     if (!c) return nullptr;
     c->params.clear();
+    c->dbounds = nullptr;
     c->local_opt = nullptr;
     c->force_stop_child = nullptr;
     c->errmsg.clear();
     c->has_errmsg = false;
     for (NamedParam *p : opt->params) c->params.push_back(new NamedParam(*p));
+    std::string err;
+    if (device_mode(opt) && !opt->dbounds->copy_into(&c->dbounds, &err)) {
+        c->munge_on_destroy = nullptr;
+        nlopt_destroy(c);
+        return nullptr;
+    }
     if (nlopt_munge mg = c->munge_on_copy) {
         bool bad = false;
         if (c->f_data && !(c->f_data = mg(c->f_data))) bad = true;
@@ -422,6 +466,7 @@ nlopt_result nlopt_set_lower_bounds(nlopt_opt opt, const double *lb)
 {
     clear_err(opt);
     if (!opt || (opt->n > 0 && !lb)) return NLOPT_INVALID_ARGS;
+    if (!leave_device_mode(opt)) return NLOPT_FAILURE;
     for (unsigned i = 0; i < opt->n; ++i) opt->lb[i] = lb[i];
     for (unsigned i = 0; i < opt->n; ++i) snap_lower(opt, i);
     opt->lb_uniform = false;
@@ -432,6 +477,7 @@ nlopt_result nlopt_set_lower_bounds1(nlopt_opt opt, double lb)
 {
     clear_err(opt);
     if (!opt) return NLOPT_INVALID_ARGS;
+    if (!leave_device_mode(opt)) return NLOPT_FAILURE;
     for (unsigned i = 0; i < opt->n; ++i) { opt->lb[i] = lb; snap_lower(opt, i); }
     opt->lb_uniform = true;
     for (unsigned i = 1; i < opt->n && opt->lb_uniform; ++i) opt->lb_uniform = opt->lb[i] == opt->lb[0];   // snapping may differ
@@ -443,6 +489,7 @@ nlopt_result nlopt_set_lower_bound(nlopt_opt opt, int i, double lb)
     clear_err(opt);
     if (!opt) return NLOPT_INVALID_ARGS;
     if (i < 0 || i >= (int) opt->n) { set_err(opt, "invalid bound index"); return NLOPT_INVALID_ARGS; }
+    if (!leave_device_mode(opt)) return NLOPT_FAILURE;
     opt->lb[i] = lb;
     snap_lower(opt, i);
     opt->lb_uniform = false;
@@ -453,6 +500,7 @@ nlopt_result nlopt_get_lower_bounds(const nlopt_opt opt, double *lb)
 {
     clear_err(opt);
     if (!opt || (opt->n > 0 && !lb)) return NLOPT_INVALID_ARGS;
+    if (!host_bounds(opt)) return NLOPT_FAILURE;
     for (unsigned i = 0; i < opt->n; ++i) lb[i] = opt->lb[i];
     return NLOPT_SUCCESS;
 }
@@ -461,6 +509,7 @@ nlopt_result nlopt_set_upper_bounds(nlopt_opt opt, const double *ub)
 {
     clear_err(opt);
     if (!opt || (opt->n > 0 && !ub)) return NLOPT_INVALID_ARGS;
+    if (!leave_device_mode(opt)) return NLOPT_FAILURE;
     for (unsigned i = 0; i < opt->n; ++i) opt->ub[i] = ub[i];
     for (unsigned i = 0; i < opt->n; ++i) snap_upper(opt, i);
     opt->ub_uniform = false;
@@ -471,6 +520,7 @@ nlopt_result nlopt_set_upper_bounds1(nlopt_opt opt, double ub)
 {
     clear_err(opt);
     if (!opt) return NLOPT_INVALID_ARGS;
+    if (!leave_device_mode(opt)) return NLOPT_FAILURE;
     for (unsigned i = 0; i < opt->n; ++i) { opt->ub[i] = ub; snap_upper(opt, i); }
     opt->ub_uniform = true;
     for (unsigned i = 1; i < opt->n && opt->ub_uniform; ++i) opt->ub_uniform = opt->ub[i] == opt->ub[0];
@@ -482,6 +532,7 @@ nlopt_result nlopt_set_upper_bound(nlopt_opt opt, int i, double ub)
     clear_err(opt);
     if (!opt) return NLOPT_INVALID_ARGS;
     if (i < 0 || i >= (int) opt->n) { set_err(opt, "invalid bound index"); return NLOPT_INVALID_ARGS; }
+    if (!leave_device_mode(opt)) return NLOPT_FAILURE;
     opt->ub[i] = ub;
     snap_upper(opt, i);
     opt->ub_uniform = false;
@@ -492,6 +543,7 @@ nlopt_result nlopt_get_upper_bounds(const nlopt_opt opt, double *ub)
 {
     clear_err(opt);
     if (!opt || (opt->n > 0 && !ub)) return NLOPT_INVALID_ARGS;
+    if (!host_bounds(opt)) return NLOPT_FAILURE;
     for (unsigned i = 0; i < opt->n; ++i) ub[i] = opt->ub[i];
     return NLOPT_SUCCESS;
 }
@@ -751,6 +803,7 @@ nlopt_result nlopt_set_local_optimizer(nlopt_opt opt, const nlopt_opt local_opt)
     if (local_opt) {
         if (!opt->local_opt) return NLOPT_OUT_OF_MEMORY;
         nlopt_opt lo = opt->local_opt;
+        if (!host_bounds(opt)) return NLOPT_FAILURE;
         nlopt_set_lower_bounds(lo, opt->lb.data());
         nlopt_set_upper_bounds(lo, opt->ub.data());
         nlopt_remove_inequality_constraints(lo);
@@ -789,6 +842,7 @@ nlopt_result nlopt_set_default_initial_step(nlopt_opt opt, const double *x)
 {
     clear_err(opt);
     if (!opt || !x) return NLOPT_INVALID_ARGS;
+    if (!host_bounds(opt)) return NLOPT_FAILURE;
     opt->dx.assign(opt->n, 1.0);
     opt->has_dx = opt->n > 0;
     for (unsigned i = 0; i < opt->n; ++i) {
@@ -989,7 +1043,9 @@ nlopt_result run_ccsa(nlopt_opt opt, double *x_host, double *x_dev, double *minf
                 nlopt_algorithm_to_string(opt->algorithm));
         return NLOPT_INVALID_ARGS;
     }
-    if (x_host)                                      /* optimize.c:547-551 */
+    const bool dev_bounds = device_mode(opt);      /* device bounds: the backend checks the start point */
+    if (dev_bounds && !device_mode_runs_here(opt)) return NLOPT_INVALID_ARGS;
+    if (x_host && !dev_bounds)                       /* optimize.c:547-551 */
         for (unsigned i = 0; i < n; ++i)
             if (opt->lb[i] > opt->ub[i] || x_host[i] < opt->lb[i] || x_host[i] > opt->ub[i]) {
                 set_err(opt, "bounds %d fail %g <= %g <= %g", (int) i, opt->lb[i], x_host[i], opt->ub[i]);
@@ -1042,6 +1098,10 @@ nlopt_result run_ccsa(nlopt_opt opt, double *x_host, double *x_dev, double *minf
             set_err(opt, "preconditioned CCSAQ takes host x and host callbacks (nlopt_precond is a host function)");
             return NLOPT_INVALID_ARGS;
         }
+        if (dev_bounds) {
+            set_err(opt, "preconditioned CCSAQ takes host bounds (its model problem is built on the host)");
+            return NLOPT_INVALID_ARGS;
+        }
         return run_ccsa_precond(opt, x_host, minf, prm);
     }
 
@@ -1071,6 +1131,13 @@ nlopt_result run_ccsa(nlopt_opt opt, double *x_host, double *x_dev, double *minf
     cfg.ub = opt->ub.data();
     cfg.lb_uniform = opt->lb_uniform && n > 0;
     cfg.ub_uniform = opt->ub_uniform && n > 0;
+    nb200::StartCheck start;
+    if (dev_bounds) {
+        cfg.lb = cfg.ub = nullptr;
+        cfg.lb_dev = opt->dbounds->lb();
+        cfg.ub_dev = opt->dbounds->ub();
+        cfg.start_check = &start;
+    }
     cfg.x0_host = x_host;
     cfg.x_dev = x_dev;
     cfg.sigma_init = opt->has_dx ? opt->dx.data() : nullptr;
@@ -1085,6 +1152,11 @@ nlopt_result run_ccsa(nlopt_opt opt, double *x_host, double *x_dev, double *minf
     if (!be) {
         set_err(opt, "%s", err.c_str());
         return NLOPT_FAILURE;
+    }
+    if (start.bad >= 0) {                            /* optimize.c:547-551, found on the device */
+        delete be;
+        set_err(opt, "bounds %d fail %g <= %g <= %g", (int) start.bad, start.lb, start.x, start.ub);
+        return NLOPT_INVALID_ARGS;
     }
     opt->stats.seconds_setup = nb200::wall_seconds() - t0;
 
@@ -1448,7 +1520,20 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
         set_err(opt, "NLOPT_AUGLAG* does not take sharded host callbacks (nlopt_b200_sfunc) in this library");
         return NLOPT_INVALID_ARGS;
     }
-    if (x)
+    const bool dev_bounds = device_mode(opt);
+    if (dev_bounds) {                                /* optimize.c:547-551 on the device, host x or device x */
+        if (!device_mode_runs_here(opt)) return NLOPT_INVALID_ARGS;
+        nb200::StartCheck start;
+        std::string err;
+        if (!opt->dbounds->check(x, x ? nullptr : x_dev, &start, &err)) {
+            set_err(opt, "%s", err.c_str());
+            return NLOPT_FAILURE;
+        }
+        if (start.bad >= 0) {
+            set_err(opt, "bounds %d fail %g <= %g <= %g", (int) start.bad, start.lb, start.x, start.ub);
+            return NLOPT_INVALID_ARGS;
+        }
+    } else if (x)
         for (unsigned i = 0; i < n; ++i)             /* optimize.c:547-551 */
             if (opt->lb[i] > opt->ub[i] || x[i] < opt->lb[i] || x[i] > opt->ub[i]) {
                 set_err(opt, "bounds %d fail %g <= %g <= %g", (int) i, opt->lb[i], x[i], opt->ub[i]);
@@ -1528,8 +1613,17 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
     sub->pre = nullptr;
     sub->maximize = 0;
     sub->negate = opt->negate;          /* a maximised device objective: the sub-problem's L starts from -f */
-    nlopt_set_lower_bounds(sub, opt->lb.data());
-    nlopt_set_upper_bounds(sub, opt->ub.data());
+    if (dev_bounds) {                                /* D2D into the sub-optimiser, which is then in device mode */
+        std::string err;
+        if (!opt->dbounds->copy_into(&sub->dbounds, &err)) {
+            set_err(opt, "%s", err.c_str());
+            return NLOPT_FAILURE;
+        }
+        sub->lb_ub_mirror = false;
+    } else {
+        nlopt_set_lower_bounds(sub, opt->lb.data());
+        nlopt_set_upper_bounds(sub, opt->ub.data());
+    }
     sub->lb_uniform = opt->lb_uniform;
     sub->ub_uniform = opt->ub_uniform;
     nlopt_set_stopval(sub, (mm == 0 && pp == 0) ? opt->stopval : -kInf);

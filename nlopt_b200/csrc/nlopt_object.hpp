@@ -7,10 +7,9 @@
 #include <vector>
 
 #include "../../include/nlopt_b200.h"
+#include "backend_factory.hpp"
 
 namespace nb200 {
-
-struct PenaltySpec;     // backend_factory.hpp
 
 // one registered constraint object (reference: nlopt_constraint, src/util/nlopt-util.h:119-126)
 struct ConstraintRec {
@@ -57,6 +56,10 @@ struct nlopt_opt_s {
 
     std::vector<double> lb, ub;
     bool lb_uniform = true, ub_uniform = true;   // every entry equal (set by nlopt_set_*_bounds1): filled on device
+    // device mode (nlopt_b200_set_*_bounds_device): both bounds live in dbounds (owned) and lb / ub hold their values
+    // only while lb_ub_mirror (after a host reader downloaded them); a host setter downloads them and leaves device mode
+    nb200::DeviceBounds *dbounds = nullptr;
+    bool lb_ub_mirror = false;
     std::vector<nb200::ConstraintRec> fc, h;      // inequality / equality constraint objects
     nlopt_munge munge_on_destroy = nullptr, munge_on_copy = nullptr;
 
