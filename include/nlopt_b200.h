@@ -33,6 +33,11 @@
  * GPU), where a run checks the start point and detects uniform bounds on the
  * device.
  *
+ * So may the per-variable options: nlopt_b200_set_xtol_abs_device,
+ * nlopt_b200_set_x_weights_device and nlopt_b200_set_initial_step_device
+ * copy n doubles from a device array and check them on the device with
+ * the host setters' rule; a run reads them in place.
+ *
  * The `nlopt_b200_*` symbols are additive extensions (device-resident
  * callbacks, kernel-level access to the dual evaluation, multi-GPU sharding,
  * statistics).  No torch / CUDA types appear in any signature: device
@@ -396,6 +401,22 @@ nlopt_result nlopt_b200_optimize_device(nlopt_opt opt, double *x_dev, double *op
  * bounds only. */
 nlopt_result nlopt_b200_set_lower_bounds_device(nlopt_opt opt, const double *lb_dev);
 nlopt_result nlopt_b200_set_upper_bounds_device(nlopt_opt opt, const double *ub_dev);
+/* xtol_abs, x_weights and the initial step (MMA / CCSAQ: each variable's first move limit, sigma_0) from device memory.
+ * Each call copies the n doubles at its argument into device memory the object owns (on the current device) and returns
+ * when the copy and its check are complete, so the buffer may be reused at once; the work that produces it must be
+ * complete before the call.  The check is the host setter's, made on the device: a negative weight gives
+ * NLOPT_INVALID_ARGS and "invalid negative weight", a zero step (+0.0 or -0.0) NLOPT_INVALID_ARGS and "zero step size"
+ * (NaN passes both); xtol_abs is not checked.  The option is then in device mode, independently of the other two and of
+ * the bounds: a run reads it in place (no host-to-device copy), and a bitwise uniform step takes the sigma index as
+ * nlopt_set_initial_step1 does.  Any host setter of the same option (nlopt_set_xtol_abs / _xtol_abs1, nlopt_set_x_weights
+ * / _x_weights1, nlopt_set_initial_step / _initial_step1, nlopt_set_default_initial_step; NULL included) frees the device
+ * copy and leaves device mode; nlopt_get_xtol_abs, nlopt_get_x_weights and nlopt_get_initial_step read the device
+ * values; nlopt_copy duplicates them; NLOPT_AUGLAG* hands the step (and xtol_abs, to a sub-optimiser it creates) to its
+ * sub-optimiser device to device.  NULL: NLOPT_INVALID_ARGS; n == 0: no-op; no usable device: NLOPT_FAILURE; several
+ * ranks, or a run on another current device: NLOPT_INVALID_ARGS.  A failed call keeps the previous values. */
+nlopt_result nlopt_b200_set_xtol_abs_device(nlopt_opt opt, const double *xtol_abs_dev);
+nlopt_result nlopt_b200_set_x_weights_device(nlopt_opt opt, const double *w_dev);
+nlopt_result nlopt_b200_set_initial_step_device(nlopt_opt opt, const double *dx_dev);
 
 /* Run statistics of the last nlopt_optimize on this object; after an NLOPT_AUGLAG* run, those of its last
  * sub-optimisation. */

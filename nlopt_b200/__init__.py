@@ -70,7 +70,7 @@ def _cuda_f64(v, n):
         step *= d
     if (cai["typestr"] != "<f8" or int(np.prod(shape, dtype=np.int64)) != n
             or (strides is not None and tuple(strides) != tuple(contiguous))):
-        raise ValueError(f"device bounds need a contiguous float64 CUDA array of {n} values (got typestr "
+        raise ValueError(f"device arrays need a contiguous float64 CUDA array of {n} values (got typestr "
                          f"{cai['typestr']}, shape {shape}, strides {strides})")
     return cai["data"][0]
 
@@ -531,10 +531,10 @@ class opt:
         self._check(fn(self._h, _ptr(a)))
         return a
 
-    # bounds: a scalar, a host array, or a device array (__cuda_array_interface__: a CUDA tensor, a CuPy array ...), which
-    # the library copies into its own device memory (nlopt_b200_set_*_bounds_device); a torch tensor's current stream is
-    # synchronised first
-    def _set_bounds(self, vec_fn, scalar_fn, dev_name, v):
+    # bounds, xtol_abs, x_weights and the initial step: a scalar, a host array, or a device array (__cuda_array_interface__:
+    # a CUDA tensor, a CuPy array ...), which the library copies into its own device memory (nlopt_b200_set_*_device); a
+    # torch tensor's current stream is synchronised first
+    def _set_array(self, vec_fn, scalar_fn, dev_name, v):
         if not hasattr(v, "__cuda_array_interface__"):
             self._set_vec_or_scalar(vec_fn, scalar_fn, v)
             return
@@ -549,12 +549,12 @@ class opt:
             self._check(dev_fn(self._h, ptr))
 
     def set_lower_bounds(self, v):
-        self._set_bounds(self._lib.nlopt_set_lower_bounds, self._lib.nlopt_set_lower_bounds1,
-                         "nlopt_b200_set_lower_bounds_device", v)
+        self._set_array(self._lib.nlopt_set_lower_bounds, self._lib.nlopt_set_lower_bounds1,
+                        "nlopt_b200_set_lower_bounds_device", v)
 
     def set_upper_bounds(self, v):
-        self._set_bounds(self._lib.nlopt_set_upper_bounds, self._lib.nlopt_set_upper_bounds1,
-                         "nlopt_b200_set_upper_bounds_device", v)
+        self._set_array(self._lib.nlopt_set_upper_bounds, self._lib.nlopt_set_upper_bounds1,
+                        "nlopt_b200_set_upper_bounds_device", v)
 
     def set_lower_bound(self, i, v):
         self._check(self._lib.nlopt_set_lower_bound(self._h, int(i), float(v)))
@@ -569,19 +569,20 @@ class opt:
         return self._get_vec(self._lib.nlopt_get_upper_bounds)
 
     def set_xtol_abs(self, v):
-        self._set_vec_or_scalar(self._lib.nlopt_set_xtol_abs, self._lib.nlopt_set_xtol_abs1, v)
+        self._set_array(self._lib.nlopt_set_xtol_abs, self._lib.nlopt_set_xtol_abs1, "nlopt_b200_set_xtol_abs_device", v)
 
     def get_xtol_abs(self):
         return self._get_vec(self._lib.nlopt_get_xtol_abs)
 
     def set_x_weights(self, v):
-        self._set_vec_or_scalar(self._lib.nlopt_set_x_weights, self._lib.nlopt_set_x_weights1, v)
+        self._set_array(self._lib.nlopt_set_x_weights, self._lib.nlopt_set_x_weights1, "nlopt_b200_set_x_weights_device", v)
 
     def get_x_weights(self):
         return self._get_vec(self._lib.nlopt_get_x_weights)
 
     def set_initial_step(self, v):
-        self._set_vec_or_scalar(self._lib.nlopt_set_initial_step, self._lib.nlopt_set_initial_step1, v)
+        self._set_array(self._lib.nlopt_set_initial_step, self._lib.nlopt_set_initial_step1,
+                        "nlopt_b200_set_initial_step_device", v)
 
     def get_initial_step(self, x):
         xa = _as_f64(x, self._n)

@@ -71,6 +71,12 @@ struct BackendConfig {
     const double *sigma_init = nullptr;      // nlopt initial step (host) or null
     const double *x_weights = nullptr;       // host or null
     const double *xtol_abs = nullptr;        // host or null
+    // ... or the same three from an object whose option is in device mode (one rank, n entries): read in place, never
+    // copied or freed by the backend.  The step's uniformity and lane 0 come from the setter's check.
+    const double *sigma_init_dev = nullptr;
+    bool sigma_init_uniform = false;         // every lane has the bits of sigma_init0
+    double sigma_init0 = 0.0;
+    const double *x_weights_dev = nullptr, *xtol_abs_dev = nullptr;
     nlopt_b200_stats *stats = nullptr;       // h2d/d2h bytes, launches, kernel time
     bool values_only = false;                // x, the best point and the callback workspace only (Backend::point_device)
 };
@@ -93,6 +99,22 @@ public:
     virtual bool runs_here(std::string *err) const = 0;
     // the start-point test against these bounds, for a start point in host memory or on the device (one of them)
     virtual bool check(const double *x_host, const double *x_dev, StartCheck *out, std::string *err) const = 0;
+};
+
+// One per-variable option of an nlopt_opt in device mode (xtol_abs, x_weights or the initial step, set by
+// nlopt_b200_set_*_device in device_backend.cu): n doubles on the device that was current at the setter, which checked
+// them with the host setter's rule.  Reached by the API layer through this interface only, as DeviceBounds.
+class DeviceVector {
+public:
+    virtual ~DeviceVector() {}
+    virtual const double *data() const = 0;
+    virtual bool uniform() const = 0;        // every lane has the bits of lane0()
+    virtual double lane0() const = 0;
+    virtual bool download(double *host, std::string *err) const = 0;
+    // *dst (allocated on this object's device when null) <- these values, device to device
+    virtual bool copy_into(DeviceVector **dst, std::string *err) const = 0;
+    // a run may use them: one rank, and their device is the current one
+    virtual bool runs_here(std::string *err) const = 0;
 };
 
 }  // namespace nb200

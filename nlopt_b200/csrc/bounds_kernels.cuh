@@ -1,5 +1,6 @@
-// bounds_kernels.cuh -- box bounds held in device memory (nlopt_b200_set_*_bounds_device): the snap of the setters and
-// the start-point check of nlopt_optimize, as element-wise kernels.  Included by device_backend.cu only.
+// bounds_kernels.cuh -- box bounds and per-variable options held in device memory (nlopt_b200_set_*_bounds_device,
+// nlopt_b200_set_{xtol_abs,x_weights,initial_step}_device): the snap of the bound setters, the start-point check of
+// nlopt_optimize and the option setters' check, as element-wise kernels.  Included by device_backend.cu only.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -69,6 +70,45 @@ __global__ void __launch_bounds__(256) bounds_check_kernel(const double *__restr
         }
         r->lb0 = lb[0];
         r->ub0 = ub[0];
+        r->done = 0;
+    }
+}
+
+// The rule of a per-variable option's host setter (options.c): x_weights refuse a negative entry, the initial step a
+// zero one (+0.0 or -0.0); xtol_abs takes any value.  NaN passes every rule, as on the host.
+enum OptionRule : int { kAnyValue = 0, kNoNegative = 1, kNoZero = 2 };
+
+// What option_check_kernel hands back; the host reads it once, with the synchronisation that ends the setter.
+struct OptionReport {
+    unsigned flags;             // bit 0: some lane fails the rule; bit 1: some lane's bits differ from lane 0's
+    unsigned done;              // CTAs finished (the last one fills v0 and rearms the counter)
+    double v0;                  // lane 0: sigma_0 of the sigma palette when the initial step is uniform
+};
+
+// One pass over a per-variable option v (nlopt_b200_set_{x_weights,initial_step,xtol_abs}_device): whether any lane
+// fails the setter's rule, and whether every lane has the bits of lane 0 (a -0.0 next to +0.0 is not uniform: a uniform
+// step hands every lane lane 0's bits, as nlopt_set_initial_step1 does).  r: flags = done = 0 on entry.
+__global__ void __launch_bounds__(256) option_check_kernel(const double *__restrict__ v, unsigned n, int rule,
+                                                           OptionReport *r)
+{
+    const long long b0 = __double_as_longlong(v[0]);
+    unsigned flags = 0;
+    for (size_t i = (size_t) blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t) gridDim.x * blockDim.x) {
+        const double x = v[i];
+        const bool bad = (rule == kNoNegative && x < 0.0) || (rule == kNoZero && x == 0.0);
+        flags |= (bad ? 1u : 0u) | (__double_as_longlong(x) != b0 ? 2u : 0u);
+    }
+    flags = __reduce_or_sync(0xffffffffu, flags);
+    if ((threadIdx.x & 31) == 0 && flags) atomicOr(&r->flags, flags);
+    __syncthreads();
+    __shared__ bool last;
+    if (threadIdx.x == 0) {
+        __threadfence();
+        last = atomicAdd(&r->done, 1u) == gridDim.x - 1;
+    }
+    __syncthreads();
+    if (last && threadIdx.x == 0) {
+        r->v0 = v[0];
         r->done = 0;
     }
 }

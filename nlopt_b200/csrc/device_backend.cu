@@ -244,8 +244,10 @@ void DeviceBackend::free_state()
     if (pool_) BlockCache::get().give(false, pool_bytes_, pool_, device_);
     if (pen_rows_) BlockCache::get().give(false, (size_t) pen_total_ * geo_.ld * sizeof(double), pen_rows_, device_);
     pen_rows_ = nullptr;
-    if (w_dev_) cudaFree(w_dev_);
-    if (xtol_abs_dev_) cudaFree(xtol_abs_dev_);
+    if (w_own_) cudaFree(w_own_);
+    if (xtol_abs_own_) cudaFree(xtol_abs_own_);
+    w_own_ = xtol_abs_own_ = nullptr;
+    w_dev_ = xtol_abs_dev_ = nullptr;
     for (const Owned &o : owned_) BlockCache::get().give(o.pinned, o.bytes, o.p, device_);   // every small buffer
     owned_.clear();
     if (xfull_dev_) BlockCache::get().give(false, (size_t) Comm::instance().world * shard_cap_ * sizeof(double), xfull_dev_, device_);
@@ -270,7 +272,7 @@ void DeviceBackend::free_state()
     }
     if (stream_) cudaStreamDestroy(stream_);
     if (copy_stream_) cudaStreamDestroy(copy_stream_);
-    pool_ = w_dev_ = xtol_abs_dev_ = partials_ = vsums_ = out_dev_ = xfull_dev_ = scalar_dev_ = nullptr;
+    pool_ = partials_ = vsums_ = out_dev_ = xfull_dev_ = scalar_dev_ = nullptr;
     tickets_ = nullptr;
     out_host_ = nullptr;
     flag_host_ = nullptr;
@@ -455,7 +457,7 @@ bool DeviceBackend::setup(const BackendConfig &cfg)
         } else
             return fail("no start point");
         NB_CUDA(cudaMemcpyAsync(xprev_, x_, nl * sizeof(double), cudaMemcpyDeviceToDevice, stream_));
-        return set_norm_arrays(cfg.x_weights, cfg.xtol_abs);
+        return set_norm_arrays(cfg.x_weights, cfg.xtol_abs, cfg.x_weights_dev, cfg.xtol_abs_dev);
     }
     if (pen_total_) {
         NB_CUDA(cached_malloc(&pen_rows_, (size_t) pen_total_ * geo_.ld * sizeof(double)));
@@ -530,7 +532,7 @@ bool DeviceBackend::setup(const BackendConfig &cfg)
         NB_CUDA(enqueue_bounds_check(lb_, ub_, x_, (unsigned) nl, rep_dev, rep_host, sm_count_, stream_));
         ++stats_->kernel_launches;
     }
-    if (!set_norm_arrays(cfg.x_weights, cfg.xtol_abs)) return false;
+    if (!set_norm_arrays(cfg.x_weights, cfg.xtol_abs, cfg.x_weights_dev, cfg.xtol_abs_dev)) return false;
     NB_CUDA(cudaStreamSynchronize(stream_));
     if (rep_host) {
         if (cfg.start_check) read_bounds_report(*rep_host, cfg.start_check);
@@ -550,18 +552,27 @@ bool DeviceBackend::setup(const BackendConfig &cfg)
     return true;
 }
 
-bool DeviceBackend::set_norm_arrays(const double *w_host, const double *xtol_abs_host)
+// Host arrays are uploaded into memory of the backend; device arrays (an object's device options, one rank) are read
+// in place.  end_outer_kernel reads lanes j < n_local only.
+bool DeviceBackend::set_norm_arrays(const double *w_host, const double *xtol_abs_host, const double *w_dev,
+                                    const double *xtol_abs_dev)
 {
     const size_t nl = geo_.n_local, j0 = geo_.j0;
-    if (w_dev_) { cudaFree(w_dev_); w_dev_ = nullptr; }
-    if (xtol_abs_dev_) { cudaFree(xtol_abs_dev_); xtol_abs_dev_ = nullptr; }
+    if (w_own_) { cudaFree(w_own_); w_own_ = nullptr; }
+    if (xtol_abs_own_) { cudaFree(xtol_abs_own_); xtol_abs_own_ = nullptr; }
+    w_dev_ = w_dev;
+    xtol_abs_dev_ = xtol_abs_dev;
     if (w_host) {
-        NB_CUDA(cudaMalloc(&w_dev_, geo_.ld * sizeof(double)));
-        NB_CUDA(cudaMemcpyAsync(w_dev_, w_host + j0, nl * sizeof(double), cudaMemcpyHostToDevice, stream_));
+        NB_CUDA(cudaMalloc(&w_own_, geo_.ld * sizeof(double)));
+        NB_CUDA(cudaMemcpyAsync(w_own_, w_host + j0, nl * sizeof(double), cudaMemcpyHostToDevice, stream_));
+        stats_->h2d_bytes += nl * sizeof(double);
+        w_dev_ = w_own_;
     }
     if (xtol_abs_host) {
-        NB_CUDA(cudaMalloc(&xtol_abs_dev_, geo_.ld * sizeof(double)));
-        NB_CUDA(cudaMemcpyAsync(xtol_abs_dev_, xtol_abs_host + j0, nl * sizeof(double), cudaMemcpyHostToDevice, stream_));
+        NB_CUDA(cudaMalloc(&xtol_abs_own_, geo_.ld * sizeof(double)));
+        NB_CUDA(cudaMemcpyAsync(xtol_abs_own_, xtol_abs_host + j0, nl * sizeof(double), cudaMemcpyHostToDevice, stream_));
+        stats_->h2d_bytes += nl * sizeof(double);
+        xtol_abs_dev_ = xtol_abs_own_;
     }
     NB_CUDA(cudaStreamSynchronize(stream_));
     return true;
@@ -572,21 +583,27 @@ bool DeviceBackend::set_norm_arrays(const double *w_host, const double *xtol_abs
 
 bool DeviceBackend::sigma_init_from(const double *sigma_init_host, double sigma_min)
 {
+    if (!sigma_init_host) return sigma_init_dev(nullptr, true, 0.0, sigma_min);
+    // xprevprev is free until the second outer iteration: use it as scratch
+    NB_CUDA(cudaMemcpyAsync(xprevprev_, sigma_init_host + geo_.j0, geo_.n_local * sizeof(double), cudaMemcpyHostToDevice, stream_));
+    stats_->h2d_bytes += geo_.n_local * sizeof(double);
+    // the same step for every variable (all of them, so that every rank decides alike); scanned only when the sigma index
+    // could run
+    bool uniform = sidx_ != nullptr && sigma_index_runs();
+    for (size_t j = 1; j < (size_t) geo_.n && uniform; ++j)
+        uniform = std::memcmp(sigma_init_host + j, sigma_init_host, sizeof(double)) == 0;
+    return sigma_init_dev(xprevprev_, uniform, sigma_init_host[0], sigma_min);
+}
+
+// init_dev: this rank's initial step on the device, or null; uniform: every lane of the whole step has the bits of init0
+bool DeviceBackend::sigma_init_dev(const double *init_dev, bool uniform, double init0, double sigma_min)
+{
     const size_t nl = geo_.n_local;
-    const double *init_dev = nullptr;
-    if (sigma_init_host) {           // xprevprev is free until the second outer iteration: use it as scratch
-        NB_CUDA(cudaMemcpyAsync(xprevprev_, sigma_init_host + geo_.j0, nl * sizeof(double), cudaMemcpyHostToDevice, stream_));
-        stats_->h2d_bytes += nl * sizeof(double);
-        init_dev = xprevprev_;
-    }
-    // the sigma index needs one sigma_0: uniform bounds, and no initial step or the same one for every variable (all of
-    // them, so that every rank decides alike); it is kept only when the solve kernel that reads it will run
-    sidx_valid_ = sidx_ != nullptr && sigma_index_runs();
-    if (sidx_valid_ && sigma_init_host)
-        for (size_t j = 1; j < (size_t) geo_.n && sidx_valid_; ++j)
-            sidx_valid_ = std::memcmp(sigma_init_host + j, sigma_init_host, sizeof(double)) == 0;
+    // the sigma index needs one sigma_0: uniform bounds, and no initial step or a uniform one; it is kept only when the
+    // solve kernel that reads it will run
+    sidx_valid_ = sidx_ != nullptr && sigma_index_runs() && uniform;
     if (sidx_valid_) {
-        palette_.reset(SigmaPalette::sigma0(lb_u_, ub_u_, sigma_init_host ? sigma_init_host[0] : 0.0, sigma_min), lb_u_, ub_u_,
+        palette_.reset(SigmaPalette::sigma0(lb_u_, ub_u_, init_dev ? init0 : 0.0, sigma_min), lb_u_, ub_u_,
                        variant_ == kMMA ? 0.01 : 1e-8, sigma_min);
         sidx_sigma_min_ = sigma_min;
         pal_uploaded_ = rows_uploaded_ = 0;
@@ -600,7 +617,11 @@ bool DeviceBackend::sigma_init_from(const double *sigma_init_host, double sigma_
     return true;
 }
 
-bool DeviceBackend::init_sigma(double sigma_min) { return sigma_init_from(cfg_.sigma_init, sigma_min); }
+bool DeviceBackend::init_sigma(double sigma_min)
+{
+    if (cfg_.sigma_init_dev) return sigma_init_dev(cfg_.sigma_init_dev, cfg_.sigma_init_uniform, cfg_.sigma_init0, sigma_min);
+    return sigma_init_from(cfg_.sigma_init, sigma_min);
+}
 
 // The sigma-index form of the TMA-staged solve kernel runs -- and only then is the index kept -- with uniform bounds,
 // 4 rows, the TMA form chosen by the default rule (knob b200_solve_tma = 1 forces the TMA form with the fp64 sigma),
@@ -1836,8 +1857,8 @@ long long DeviceBackend::query(const char *key) const
 void release_cached_blocks() { BlockCache::get().clear(); }
 
 // ------------------------------------------------------------------------------------------------
-// bounds of an object in device mode.  The work goes to the per-thread default stream and is complete on return, so a
-// caller may reuse its buffers at once (NLopt's copy semantics).
+// bounds and per-variable options of an object in device mode.  The work goes to the per-thread default stream and is
+// complete on return, so a caller may reuse its buffers at once (NLopt's copy semantics).
 
 namespace {
 
@@ -1861,21 +1882,24 @@ struct DeviceGuard {
     }
 };
 
-class DeviceBoundsImpl : public DeviceBounds {
+// what: "bounds (nlopt_b200_set_*_bounds_device)", ...: the refusal of a device-mode array while several ranks run
+std::string one_rank_message(const char *what) { return std::string("device ") + what + " run on one rank in this library"; }
+
+// Device memory of an object in device mode: `count` doubles on the device that was current at alloc(), freed there.
+// Device bounds and device options both keep their values in one of these.
+class DeviceStore {
 public:
-    explicit DeviceBoundsImpl(unsigned n) : n_(n) {}
-    ~DeviceBoundsImpl() override
+    ~DeviceStore()
     {
         if (p_) {
             DeviceGuard g(device_);
             cudaFree(p_);
         }
     }
-    const double *lb() const override { return p_; }
-    const double *ub() const override { return p_ + n_; }
+    double *data() const { return p_; }
+    int device() const { return device_; }
 
-    // both arrays on the current device
-    bool alloc(std::string *err)
+    bool alloc(size_t count, std::string *err)
     {
         int ndev = 0;
         const cudaError_t e = cudaGetDeviceCount(&ndev);
@@ -1883,73 +1907,108 @@ public:
             *err = no_device_message(e);
             return false;
         }
+        count_ = count;
         return cuda_ok(cudaGetDevice(&device_), "cudaGetDevice", err) &&
-               cuda_ok(cudaMalloc(&p_, 2 * bytes()), "cudaMalloc", err);
+               cuda_ok(cudaMalloc(&p_, count * sizeof(double)), "cudaMalloc", err);
     }
-    // lb / ub <- lb_src / ub_src (any memory CUDA can read; null: keep)
-    bool upload(const double *lb_src, const double *ub_src, std::string *err)
+    // [off, off + count) <- src (any memory CUDA can read); enqueued only
+    bool put(size_t off, const double *src, size_t count, std::string *err)
     {
-        return (!lb_src || cuda_ok(cudaMemcpyAsync(p_, lb_src, bytes(), cudaMemcpyDefault, cudaStreamPerThread), "cudaMemcpyAsync", err)) &&
-               (!ub_src || cuda_ok(cudaMemcpyAsync(p_ + n_, ub_src, bytes(), cudaMemcpyDefault, cudaStreamPerThread), "cudaMemcpyAsync", err)) &&
-               cuda_ok(cudaStreamSynchronize(cudaStreamPerThread), "cudaStreamSynchronize", err);
+        return cuda_ok(cudaMemcpyAsync(p_ + off, src, count * sizeof(double), cudaMemcpyDefault, cudaStreamPerThread),
+                       "cudaMemcpyAsync", err);
     }
-    // the caller's n doubles into the lower (or upper) array, then the setters' snap against the other one
-    bool set(bool lower, const double *src, std::string *err)
+    bool download(size_t off, double *dst, size_t count, std::string *err) const
     {
-        DeviceGuard g(device_);
-        double *dst = lower ? p_ : p_ + n_;
-        int sms = 0;
-        if (!cuda_ok(cudaMemcpyAsync(dst, src, bytes(), cudaMemcpyDefault, cudaStreamPerThread), "cudaMemcpyAsync", err) ||
-            !cuda_ok(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device_), "cudaDeviceGetAttribute", err))
-            return false;
-        snap_bounds_kernel<<<grid_for(n_, sms), kBlock, 0, cudaStreamPerThread>>>(dst, lower ? p_ + n_ : p_, lower, n_);
-        return cuda_ok(cudaGetLastError(), "snap_bounds_kernel", err) &&
-               cuda_ok(cudaStreamSynchronize(cudaStreamPerThread), "cudaStreamSynchronize", err);
+        return cuda_ok(cudaMemcpyAsync(dst, p_ + off, count * sizeof(double), cudaMemcpyDefault, cudaStreamPerThread),
+                       "cudaMemcpyAsync", err) &&
+               sync(err);
     }
-    bool download(double *lb_host, double *ub_host, std::string *err) const override
-    {
-        return cuda_ok(cudaMemcpyAsync(lb_host, p_, bytes(), cudaMemcpyDefault, cudaStreamPerThread), "cudaMemcpyAsync", err) &&
-               cuda_ok(cudaMemcpyAsync(ub_host, p_ + n_, bytes(), cudaMemcpyDefault, cudaStreamPerThread), "cudaMemcpyAsync", err) &&
-               cuda_ok(cudaStreamSynchronize(cudaStreamPerThread), "cudaStreamSynchronize", err);
-    }
-    bool copy_into(DeviceBounds **dst, std::string *err) const override
+    // dst (allocated on this store's device when empty) <- every value, device to device
+    bool copy_into(DeviceStore &dst, std::string *err) const
     {
         DeviceGuard g(device_);
-        if (!*dst) {
-            DeviceBoundsImpl *d = new DeviceBoundsImpl(n_);
-            if (!d->alloc(err)) {
-                delete d;
-                return false;
-            }
-            *dst = d;
-        }
-        DeviceBoundsImpl *d = static_cast<DeviceBoundsImpl *>(*dst);
-        return cuda_ok(cudaMemcpyAsync(d->p_, p_, 2 * bytes(), cudaMemcpyDefault, cudaStreamPerThread), "cudaMemcpyAsync", err) &&
-               cuda_ok(cudaStreamSynchronize(cudaStreamPerThread), "cudaStreamSynchronize", err);
+        return (dst.p_ || dst.alloc(count_, err)) &&
+               cuda_ok(cudaMemcpyAsync(dst.p_, p_, count_ * sizeof(double), cudaMemcpyDefault, cudaStreamPerThread),
+                       "cudaMemcpyAsync", err) &&
+               sync(err);
     }
-    bool runs_here(std::string *err) const override
+    // a run may use the values: one rank, and their device is the current one
+    bool runs_here(const char *what, const char *name, std::string *err) const
     {
         if (Comm::instance().active()) {
-            *err = "device bounds (nlopt_b200_set_*_bounds_device) run on one rank in this library";
+            *err = one_rank_message(what);
             return false;
         }
         int d = -1;
         cudaGetDevice(&d);
         if (d != device_) {
-            *err = "the device bounds live on CUDA device " + std::to_string(device_) + " but device " + std::to_string(d) +
-                   " is current";
+            *err = std::string("the device ") + name + " live on CUDA device " + std::to_string(device_) + " but device " +
+                   std::to_string(d) + " is current";
             return false;
         }
         return true;
     }
+    static bool sync(std::string *err)
+    {
+        return cuda_ok(cudaStreamSynchronize(cudaStreamPerThread), "cudaStreamSynchronize", err);
+    }
+
+private:
+    size_t count_ = 0;
+    int device_ = -1;
+    double *p_ = nullptr;
+};
+
+const char *const kBoundsWhat = "bounds (nlopt_b200_set_*_bounds_device)";
+
+class DeviceBoundsImpl : public DeviceBounds {
+public:
+    explicit DeviceBoundsImpl(unsigned n) : n_(n) {}
+    const double *lb() const override { return mem_.data(); }
+    const double *ub() const override { return mem_.data() + n_; }
+
+    // both arrays on the current device
+    bool alloc(std::string *err) { return mem_.alloc(2 * (size_t) n_, err); }
+    // lb / ub <- lb_src / ub_src (any memory CUDA can read; null: keep)
+    bool upload(const double *lb_src, const double *ub_src, std::string *err)
+    {
+        return (!lb_src || mem_.put(0, lb_src, n_, err)) && (!ub_src || mem_.put(n_, ub_src, n_, err)) &&
+               DeviceStore::sync(err);
+    }
+    // the caller's n doubles into the lower (or upper) array, then the setters' snap against the other one
+    bool set(bool lower, const double *src, std::string *err)
+    {
+        DeviceGuard g(mem_.device());
+        double *dst = lower ? mem_.data() : mem_.data() + n_;
+        int sms = 0;
+        if (!mem_.put(lower ? 0 : n_, src, n_, err) ||
+            !cuda_ok(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, mem_.device()), "cudaDeviceGetAttribute", err))
+            return false;
+        snap_bounds_kernel<<<grid_for(n_, sms), kBlock, 0, cudaStreamPerThread>>>(dst, lower ? dst + n_ : mem_.data(), lower, n_);
+        return cuda_ok(cudaGetLastError(), "snap_bounds_kernel", err) && DeviceStore::sync(err);
+    }
+    bool download(double *lb_host, double *ub_host, std::string *err) const override
+    {
+        return mem_.download(0, lb_host, n_, err) && mem_.download(n_, ub_host, n_, err);
+    }
+    bool copy_into(DeviceBounds **dst, std::string *err) const override
+    {
+        std::unique_ptr<DeviceBoundsImpl> fresh(*dst ? nullptr : new DeviceBoundsImpl(n_));
+        DeviceBoundsImpl *d = fresh ? fresh.get() : static_cast<DeviceBoundsImpl *>(*dst);
+        if (!mem_.copy_into(d->mem_, err)) return false;
+        if (fresh) *dst = fresh.release();
+        return true;
+    }
+    bool runs_here(std::string *err) const override { return mem_.runs_here(kBoundsWhat, "bounds", err); }
     bool check(const double *x_host, const double *x_dev, StartCheck *out, std::string *err) const override
     {
-        DeviceGuard g(device_);
+        const int device = mem_.device();
+        DeviceGuard g(device);
         const cudaStream_t s = cudaStreamPerThread;
         BoundsReport *rep_dev = nullptr, *rep_host = nullptr;
         double *x_stage = nullptr;
         int sms = 0;
-        bool good = cuda_ok(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device_), "cudaDeviceGetAttribute", err) &&
+        bool good = cuda_ok(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device), "cudaDeviceGetAttribute", err) &&
                     cuda_ok(cached_malloc((double **) &rep_dev, sizeof(BoundsReport)), "cudaMalloc", err) &&
                     cuda_ok(cached_host_alloc((double **) &rep_host, sizeof(BoundsReport)), "cudaHostAlloc", err);
         if (good && x_host) {
@@ -1961,8 +2020,8 @@ public:
                cuda_ok(cudaStreamSynchronize(s), "cudaStreamSynchronize", err);
         if (good) read_bounds_report(*rep_host, out);
         cudaStreamSynchronize(s);
-        if (x_stage) BlockCache::get().give(false, bytes(), x_stage, device_);
-        if (rep_dev) BlockCache::get().give(false, sizeof(BoundsReport), rep_dev, device_);
+        if (x_stage) BlockCache::get().give(false, bytes(), x_stage, device);
+        if (rep_dev) BlockCache::get().give(false, sizeof(BoundsReport), rep_dev, device);
         if (rep_host) BlockCache::get().give(true, sizeof(BoundsReport), rep_host);
         return good;
     }
@@ -1970,8 +2029,65 @@ public:
 private:
     size_t bytes() const { return (size_t) n_ * sizeof(double); }
     unsigned n_;
-    int device_ = -1;
-    double *p_ = nullptr;            // lb | ub
+    DeviceStore mem_;                // lb | ub
+};
+
+// xtol_abs, x_weights or the initial step of an object in device mode
+class DeviceVectorImpl : public DeviceVector {
+public:
+    // what: "xtol_abs (nlopt_b200_set_xtol_abs_device)" ..., name: "xtol_abs" ... (messages)
+    DeviceVectorImpl(unsigned n, const char *what, const char *name) : n_(n), what_(what), name_(name) {}
+    const double *data() const override { return mem_.data(); }
+    bool uniform() const override { return uniform_; }
+    double lane0() const override { return lane0_; }
+
+    // the caller's n doubles into fresh memory on the current device, then option_check_kernel with the setter's rule:
+    // *rejected when a lane fails it
+    bool set(const double *src, OptionRule rule, bool *rejected, std::string *err)
+    {
+        const cudaStream_t s = cudaStreamPerThread;
+        OptionReport *rep_dev = nullptr, *rep_host = nullptr;
+        int sms = 0;
+        if (!mem_.alloc(n_, err) || !mem_.put(0, src, n_, err)) return false;
+        bool good = cuda_ok(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, mem_.device()), "cudaDeviceGetAttribute", err) &&
+                    cuda_ok(cached_malloc((double **) &rep_dev, sizeof(OptionReport)), "cudaMalloc", err) &&
+                    cuda_ok(cached_host_alloc((double **) &rep_host, sizeof(OptionReport)), "cudaHostAlloc", err) &&
+                    cuda_ok(cudaMemsetAsync(rep_dev, 0, sizeof(OptionReport), s), "cudaMemsetAsync", err);
+        if (good) {
+            option_check_kernel<<<grid_for(n_, sms), kBlock, 0, s>>>(mem_.data(), n_, rule, rep_dev);
+            good = cuda_ok(cudaGetLastError(), "option_check_kernel", err) &&
+                   cuda_ok(cudaMemcpyAsync(rep_host, rep_dev, sizeof(OptionReport), cudaMemcpyDeviceToHost, s), "cudaMemcpyAsync", err) &&
+                   DeviceStore::sync(err);
+        }
+        if (good) {
+            *rejected = (rep_host->flags & 1u) != 0;
+            uniform_ = (rep_host->flags & 2u) == 0;
+            lane0_ = rep_host->v0;
+        }
+        cudaStreamSynchronize(s);
+        if (rep_dev) BlockCache::get().give(false, sizeof(OptionReport), rep_dev, mem_.device());
+        if (rep_host) BlockCache::get().give(true, sizeof(OptionReport), rep_host);
+        return good;
+    }
+    bool download(double *host, std::string *err) const override { return mem_.download(0, host, n_, err); }
+    bool copy_into(DeviceVector **dst, std::string *err) const override
+    {
+        std::unique_ptr<DeviceVectorImpl> fresh(*dst ? nullptr : new DeviceVectorImpl(n_, what_, name_));
+        DeviceVectorImpl *d = fresh ? fresh.get() : static_cast<DeviceVectorImpl *>(*dst);
+        if (!mem_.copy_into(d->mem_, err)) return false;
+        d->uniform_ = uniform_;
+        d->lane0_ = lane0_;
+        if (fresh) *dst = fresh.release();
+        return true;
+    }
+    bool runs_here(std::string *err) const override { return mem_.runs_here(what_, name_, err); }
+
+private:
+    unsigned n_;
+    const char *what_, *name_;
+    DeviceStore mem_;
+    bool uniform_ = false;
+    double lane0_ = 0.0;
 };
 
 }  // namespace
@@ -2201,32 +2317,45 @@ int nlopt_b200_device_count(void)
 
 void nlopt_b200_release_cached_memory(void) { nb200::release_cached_blocks(); }
 
+/* the errmsg of a refused device setter */
+static nlopt_result refuse(nlopt_opt opt, nlopt_result r, const std::string &msg)
+{
+    opt->errmsg = msg;
+    opt->has_errmsg = true;
+    return r;
+}
+
+/* the checks every device setter starts with: true, with the result in *r, when the call ends there */
+static bool device_setter_ends(nlopt_opt opt, const double *src, const char *what, nlopt_result *r)
+{
+    *r = NLOPT_INVALID_ARGS;
+    if (!opt) return true;
+    opt->errmsg.clear();
+    opt->has_errmsg = false;
+    if (!src) return true;
+    *r = NLOPT_SUCCESS;
+    if (opt->n == 0) return true;
+    if (!nb200::Comm::instance().active()) return false;
+    *r = refuse(opt, NLOPT_INVALID_ARGS, nb200::one_rank_message(what));
+    return true;
+}
+
 /* device bounds (the rest of the bounds API is in nlopt_api.cpp).  An object whose first device setter fails keeps its
    host bounds. */
 static nlopt_result set_bounds_device(nlopt_opt opt, const double *src, bool lower)
 {
-    if (!opt) return NLOPT_INVALID_ARGS;
-    opt->errmsg.clear();
-    opt->has_errmsg = false;
-    if (!src) return NLOPT_INVALID_ARGS;
-    if (opt->n == 0) return NLOPT_SUCCESS;
-    auto refuse = [opt](nlopt_result r, const std::string &msg) {
-        opt->errmsg = msg;
-        opt->has_errmsg = true;
-        return r;
-    };
-    if (nb200::Comm::instance().active())
-        return refuse(NLOPT_INVALID_ARGS, "device bounds (nlopt_b200_set_*_bounds_device) run on one rank in this library");
+    nlopt_result r;
+    if (device_setter_ends(opt, src, nb200::kBoundsWhat, &r)) return r;
     std::string err;
     std::unique_ptr<nb200::DeviceBoundsImpl> fresh;
     nb200::DeviceBoundsImpl *b = static_cast<nb200::DeviceBoundsImpl *>(opt->dbounds);
     if (!b) {                                /* entering device mode: the other array goes up once */
         fresh.reset(new nb200::DeviceBoundsImpl(opt->n));
         if (!fresh->alloc(&err) || !fresh->upload(lower ? nullptr : opt->lb.data(), lower ? opt->ub.data() : nullptr, &err))
-            return refuse(NLOPT_FAILURE, err);
+            return refuse(opt, NLOPT_FAILURE, err);
         b = fresh.get();
     }
-    if (!b->set(lower, src, &err)) return refuse(NLOPT_FAILURE, err);
+    if (!b->set(lower, src, &err)) return refuse(opt, NLOPT_FAILURE, err);
     if (fresh) opt->dbounds = fresh.release();
     opt->lb_ub_mirror = false;
     (lower ? opt->lb_uniform : opt->ub_uniform) = false;
@@ -2235,6 +2364,46 @@ static nlopt_result set_bounds_device(nlopt_opt opt, const double *src, bool low
 
 nlopt_result nlopt_b200_set_lower_bounds_device(nlopt_opt opt, const double *lb_dev) { return set_bounds_device(opt, lb_dev, true); }
 nlopt_result nlopt_b200_set_upper_bounds_device(nlopt_opt opt, const double *ub_dev) { return set_bounds_device(opt, ub_dev, false); }
+
+/* a per-variable option from device memory (the host setters, getters and the run paths are in nlopt_api.cpp): copied
+   into fresh device memory and checked there with the host setter's rule; the object's previous values (host or
+   device) stay unless every lane passes. */
+static nlopt_result set_option_device(nlopt_opt opt, const double *src, nb200::DeviceOption nlopt_opt_s::*slot,
+                                      bool nlopt_opt_s::*has, nb200::OptionRule rule, const char *what, const char *name,
+                                      const char *rejected_msg)
+{
+    nlopt_result r;
+    if (device_setter_ends(opt, src, what, &r)) return r;
+    std::string err;
+    bool rejected = false;
+    std::unique_ptr<nb200::DeviceVectorImpl> fresh(new nb200::DeviceVectorImpl(opt->n, what, name));
+    if (!fresh->set(src, rule, &rejected, &err)) return refuse(opt, NLOPT_FAILURE, err);
+    if (rejected) return refuse(opt, NLOPT_INVALID_ARGS, rejected_msg);
+    nb200::DeviceOption &d = opt->*slot;
+    delete d.dev;
+    d.dev = fresh.release();
+    d.mirror = false;
+    opt->*has = true;
+    return NLOPT_SUCCESS;
+}
+
+nlopt_result nlopt_b200_set_xtol_abs_device(nlopt_opt opt, const double *xtol_abs_dev)
+{
+    return set_option_device(opt, xtol_abs_dev, &nlopt_opt_s::xtol_abs_dev, &nlopt_opt_s::has_xtol_abs, nb200::kAnyValue,
+                             "xtol_abs (nlopt_b200_set_xtol_abs_device)", "xtol_abs", nullptr);
+}
+
+nlopt_result nlopt_b200_set_x_weights_device(nlopt_opt opt, const double *w_dev)
+{
+    return set_option_device(opt, w_dev, &nlopt_opt_s::x_weights_dev, &nlopt_opt_s::has_x_weights, nb200::kNoNegative,
+                             "x_weights (nlopt_b200_set_x_weights_device)", "x_weights", "invalid negative weight");
+}
+
+nlopt_result nlopt_b200_set_initial_step_device(nlopt_opt opt, const double *dx_dev)
+{
+    return set_option_device(opt, dx_dev, &nlopt_opt_s::dx_dev, &nlopt_opt_s::has_dx, nb200::kNoZero,
+                             "initial steps (nlopt_b200_set_initial_step_device)", "initial steps", "zero step size");
+}
 
 const char *nlopt_b200_build_info(void)
 {

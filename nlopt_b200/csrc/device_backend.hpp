@@ -68,7 +68,9 @@ public:
     bool download(const char *which, double *host);
     bool fill_synthetic(unsigned long long seed);
     bool sigma_init_from(const double *sigma_init_host, double sigma_min);
-    bool set_norm_arrays(const double *x_weights_host, const double *xtol_abs_host);
+    bool sigma_init_dev(const double *init_dev, bool uniform, double init0, double sigma_min);
+    bool set_norm_arrays(const double *x_weights_host, const double *xtol_abs_host, const double *x_weights_dev = nullptr,
+                         const double *xtol_abs_dev = nullptr);
     bool time_dual(const double *y, const DualScalars &sc, bool materialize, int iters, double *ms_avg);
     bool configure(const char *key, long long value) override;
     long long query(const char *key) const;
@@ -143,7 +145,8 @@ private:
     size_t pool_bytes_ = 0;
     double *x_ = nullptr, *xcur_ = nullptr, *xprev_ = nullptr, *xprevprev_ = nullptr, *lb_ = nullptr, *ub_ = nullptr,
            *sigma_ = nullptr, *g_ = nullptr, *gcur_ = nullptr, *G_ = nullptr, *Gcur_ = nullptr;
-    double *w_dev_ = nullptr, *xtol_abs_dev_ = nullptr;
+    const double *w_dev_ = nullptr, *xtol_abs_dev_ = nullptr;     // what end_outer_kernel reads: an upload below, or borrowed
+    double *w_own_ = nullptr, *xtol_abs_own_ = nullptr;           // uploads of host arrays (set_norm_arrays)
     bool cand_in_x_ = true;       // the latest candidate's values live in x_ (start point / just accepted)
 
     // reduction workspace + result mailbox

@@ -96,6 +96,60 @@ bool device_mode_runs_here(nlopt_opt o)
     return false;
 }
 
+// Every host reader of a per-variable option (xtol_abs, x_weights, dx) goes through here: in device mode one download
+// into the option's host vector, which stays valid until a device setter replaces the device values; false (with a
+// message) when the download fails.
+bool host_option(nlopt_opt o, nb200::DeviceOption &d, std::vector<double> &v)
+{
+    if (!d.dev || d.mirror) return true;
+    v.resize(o->n);
+    std::string err;
+    if (!d.dev->download(v.data(), &err)) {
+        set_err(o, "%s", err.c_str());
+        return false;
+    }
+    d.mirror = true;
+    return true;
+}
+
+bool host_options(nlopt_opt o)
+{
+    return host_option(o, o->xtol_abs_dev, o->xtol_abs) && host_option(o, o->x_weights_dev, o->x_weights) &&
+           host_option(o, o->dx_dev, o->dx);
+}
+
+// a host setter of the option: the device copy goes
+void leave_device_option(nb200::DeviceOption &d)
+{
+    delete d.dev;
+    d = nb200::DeviceOption();
+}
+
+// a run with device options: one rank, on the device that holds them
+bool device_options_run_here(nlopt_opt o)
+{
+    std::string err;
+    for (const nb200::DeviceOption *d : {&o->xtol_abs_dev, &o->x_weights_dev, &o->dx_dev})
+        if (d->dev && !d->dev->runs_here(&err)) {
+            set_err(o, "%s", err.c_str());
+            return false;
+        }
+    return true;
+}
+
+// to (an option of another object) <- from, device to device; `to` is then in device mode
+bool copy_device_option(nlopt_opt o, const nb200::DeviceOption &from, nb200::DeviceOption &to, bool &to_has)
+{
+    std::string err;
+    if (!from.dev->copy_into(&to.dev, &err)) {
+        set_err(o, "%s", err.c_str());
+        return false;
+    }
+    to.mirror = false;
+    to_has = true;
+    return true;
+}
+
 bool is_auglag(nlopt_algorithm a)
 {
     return a == NLOPT_AUGLAG || a == NLOPT_AUGLAG_EQ || a == NLOPT_LN_AUGLAG || a == NLOPT_LN_AUGLAG_EQ
@@ -292,6 +346,7 @@ void nlopt_destroy(nlopt_opt opt)
     for (NamedParam *p : opt->params) delete p;
     nlopt_destroy(opt->local_opt);
     delete opt->dbounds;
+    for (nb200::DeviceOption *d : {&opt->xtol_abs_dev, &opt->x_weights_dev, &opt->dx_dev}) delete d->dev;
     delete opt;
 }
 
@@ -302,13 +357,17 @@ nlopt_opt nlopt_copy(const nlopt_opt opt)
     if (!c) return nullptr;
     c->params.clear();
     c->dbounds = nullptr;
+    c->xtol_abs_dev.dev = c->x_weights_dev.dev = c->dx_dev.dev = nullptr;
     c->local_opt = nullptr;
     c->force_stop_child = nullptr;
     c->errmsg.clear();
     c->has_errmsg = false;
     for (NamedParam *p : opt->params) c->params.push_back(new NamedParam(*p));
     std::string err;
-    if (device_mode(opt) && !opt->dbounds->copy_into(&c->dbounds, &err)) {
+    bool copied = !device_mode(opt) || opt->dbounds->copy_into(&c->dbounds, &err);
+    for (auto slot : {&nlopt_opt_s::xtol_abs_dev, &nlopt_opt_s::x_weights_dev, &nlopt_opt_s::dx_dev})
+        copied = copied && (!(opt->*slot).dev || (opt->*slot).dev->copy_into(&(c->*slot).dev, &err));
+    if (!copied) {
         c->munge_on_destroy = nullptr;
         nlopt_destroy(c);
         return nullptr;
@@ -723,6 +782,7 @@ nlopt_result nlopt_set_xtol_abs(nlopt_opt opt, const double *v)
 {
     if (!opt) return NLOPT_INVALID_ARGS;
     clear_err(opt);
+    leave_device_option(opt->xtol_abs_dev);
     if (!v) { opt->xtol_abs.clear(); opt->has_xtol_abs = false; return NLOPT_SUCCESS; }
     opt->xtol_abs.assign(v, v + opt->n);
     opt->has_xtol_abs = opt->n > 0;
@@ -733,6 +793,7 @@ nlopt_result nlopt_set_xtol_abs1(nlopt_opt opt, double v)
 {
     if (!opt) return NLOPT_INVALID_ARGS;
     clear_err(opt);
+    leave_device_option(opt->xtol_abs_dev);
     opt->xtol_abs.assign(opt->n, v);
     opt->has_xtol_abs = opt->n > 0;
     return NLOPT_SUCCESS;
@@ -742,6 +803,7 @@ nlopt_result nlopt_get_xtol_abs(const nlopt_opt opt, double *v)
 {
     clear_err(opt);
     if (!opt || (opt->n > 0 && !v)) return NLOPT_INVALID_ARGS;
+    if (!host_option(opt, opt->xtol_abs_dev, opt->xtol_abs)) return NLOPT_FAILURE;
     for (unsigned i = 0; i < opt->n; ++i) v[i] = opt->has_xtol_abs ? opt->xtol_abs[i] : 0.0;
     return NLOPT_SUCCESS;
 }
@@ -750,9 +812,15 @@ nlopt_result nlopt_set_x_weights(nlopt_opt opt, const double *w)
 {
     if (!opt) return NLOPT_INVALID_ARGS;
     clear_err(opt);
-    if (!w) { opt->x_weights.clear(); opt->has_x_weights = false; return NLOPT_SUCCESS; }
+    if (!w) {
+        leave_device_option(opt->x_weights_dev);
+        opt->x_weights.clear();
+        opt->has_x_weights = false;
+        return NLOPT_SUCCESS;
+    }
     for (unsigned i = 0; i < opt->n; ++i)
         if (w[i] < 0) { set_err(opt, "invalid negative weight"); return NLOPT_INVALID_ARGS; }
+    leave_device_option(opt->x_weights_dev);
     opt->x_weights.assign(w, w + opt->n);
     opt->has_x_weights = opt->n > 0;
     return NLOPT_SUCCESS;
@@ -763,6 +831,7 @@ nlopt_result nlopt_set_x_weights1(nlopt_opt opt, double w)
     if (!opt) return NLOPT_INVALID_ARGS;
     if (w < 0) { set_err(opt, "invalid negative weight"); return NLOPT_INVALID_ARGS; }
     clear_err(opt);
+    leave_device_option(opt->x_weights_dev);
     opt->x_weights.assign(opt->n, w);
     opt->has_x_weights = opt->n > 0;
     return NLOPT_SUCCESS;
@@ -773,6 +842,7 @@ nlopt_result nlopt_get_x_weights(const nlopt_opt opt, double *w)
     if (!opt) return NLOPT_INVALID_ARGS;
     if (opt->n > 0 && !w) { set_err(opt, "invalid NULL weights"); return NLOPT_INVALID_ARGS; }
     clear_err(opt);
+    if (!host_option(opt, opt->x_weights_dev, opt->x_weights)) return NLOPT_FAILURE;
     for (unsigned i = 0; i < opt->n; ++i) w[i] = opt->has_x_weights ? opt->x_weights[i] : 1.0;
     return NLOPT_SUCCESS;
 }
@@ -820,6 +890,7 @@ nlopt_result nlopt_set_initial_step1(nlopt_opt opt, double dx)
     if (!opt) return NLOPT_INVALID_ARGS;
     clear_err(opt);
     if (dx == 0) { set_err(opt, "zero step size"); return NLOPT_INVALID_ARGS; }
+    leave_device_option(opt->dx_dev);
     opt->dx.assign(opt->n, dx);
     opt->has_dx = opt->n > 0;
     return NLOPT_SUCCESS;
@@ -829,9 +900,15 @@ nlopt_result nlopt_set_initial_step(nlopt_opt opt, const double *dx)
 {
     if (!opt) return NLOPT_INVALID_ARGS;
     clear_err(opt);
-    if (!dx) { opt->dx.clear(); opt->has_dx = false; return NLOPT_SUCCESS; }
+    if (!dx) {
+        leave_device_option(opt->dx_dev);
+        opt->dx.clear();
+        opt->has_dx = false;
+        return NLOPT_SUCCESS;
+    }
     for (unsigned i = 0; i < opt->n; ++i)
         if (dx[i] == 0) { set_err(opt, "zero step size"); return NLOPT_INVALID_ARGS; }
+    leave_device_option(opt->dx_dev);
     opt->dx.assign(dx, dx + opt->n);
     opt->has_dx = opt->n > 0;
     return NLOPT_SUCCESS;
@@ -843,6 +920,7 @@ nlopt_result nlopt_set_default_initial_step(nlopt_opt opt, const double *x)
     clear_err(opt);
     if (!opt || !x) return NLOPT_INVALID_ARGS;
     if (!host_bounds(opt)) return NLOPT_FAILURE;
+    leave_device_option(opt->dx_dev);
     opt->dx.assign(opt->n, 1.0);
     opt->has_dx = opt->n > 0;
     for (unsigned i = 0; i < opt->n; ++i) {
@@ -874,8 +952,10 @@ nlopt_result nlopt_get_initial_step(const nlopt_opt opt, const double *x, double
         for (unsigned i = 0; i < opt->n; ++i) dx[i] = opt->dx[i];
         opt->dx.clear();                 /* x-dependent: not remembered (options.c:896-898) */
         opt->has_dx = false;
-    } else
+    } else {
+        if (!host_option(opt, opt->dx_dev, opt->dx)) return NLOPT_FAILURE;
         for (unsigned i = 0; i < opt->n; ++i) dx[i] = opt->dx[i];
+    }
     return NLOPT_SUCCESS;
 }
 
@@ -1045,6 +1125,7 @@ nlopt_result run_ccsa(nlopt_opt opt, double *x_host, double *x_dev, double *minf
     }
     const bool dev_bounds = device_mode(opt);      /* device bounds: the backend checks the start point */
     if (dev_bounds && !device_mode_runs_here(opt)) return NLOPT_INVALID_ARGS;
+    if (!device_options_run_here(opt)) return NLOPT_INVALID_ARGS;
     if (x_host && !dev_bounds)                       /* optimize.c:547-551 */
         for (unsigned i = 0; i < n; ++i)
             if (opt->lb[i] > opt->ub[i] || x_host[i] < opt->lb[i] || x_host[i] > opt->ub[i]) {
@@ -1102,6 +1183,7 @@ nlopt_result run_ccsa(nlopt_opt opt, double *x_host, double *x_dev, double *minf
             set_err(opt, "preconditioned CCSAQ takes host bounds (its model problem is built on the host)");
             return NLOPT_INVALID_ARGS;
         }
+        if (!host_options(opt)) return NLOPT_FAILURE;     /* device options: read through their host mirrors */
         return run_ccsa_precond(opt, x_host, minf, prm);
     }
 
@@ -1143,6 +1225,20 @@ nlopt_result run_ccsa(nlopt_opt opt, double *x_host, double *x_dev, double *minf
     cfg.sigma_init = opt->has_dx ? opt->dx.data() : nullptr;
     cfg.x_weights = opt->has_x_weights ? opt->x_weights.data() : nullptr;
     cfg.xtol_abs = opt->has_xtol_abs ? opt->xtol_abs.data() : nullptr;
+    if (const nb200::DeviceVector *d = opt->dx_dev.dev) {       /* device options: read in place */
+        cfg.sigma_init = nullptr;
+        cfg.sigma_init_dev = d->data();
+        cfg.sigma_init_uniform = d->uniform();
+        cfg.sigma_init0 = d->lane0();
+    }
+    if (opt->x_weights_dev.dev) {
+        cfg.x_weights = nullptr;
+        cfg.x_weights_dev = opt->x_weights_dev.dev->data();
+    }
+    if (opt->xtol_abs_dev.dev) {
+        cfg.xtol_abs = nullptr;
+        cfg.xtol_abs_dev = opt->xtol_abs_dev.dev->data();
+    }
     opt->stats = nlopt_b200_stats{};
     cfg.stats = &opt->stats;
 
@@ -1539,6 +1635,7 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
                 set_err(opt, "bounds %d fail %g <= %g <= %g", (int) i, opt->lb[i], x[i], opt->ub[i]);
                 return NLOPT_INVALID_ARGS;
             }
+    if (!device_options_run_here(opt)) return NLOPT_INVALID_ARGS;
     if ((alg == NLOPT_AUGLAG || alg == NLOPT_AUGLAG_EQ) && !opt->local_opt) {
         set_err(opt, "local optimizer must be specified for AUGLAG");
         return NLOPT_INVALID_ARGS;
@@ -1555,7 +1652,6 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
         nlopt_set_ftol_rel(sub, opt->ftol_rel);
         nlopt_set_ftol_abs(sub, opt->ftol_abs);
         nlopt_set_xtol_rel(sub, opt->xtol_rel);
-        if (opt->has_xtol_abs) nlopt_set_xtol_abs(sub, opt->xtol_abs.data());
         nlopt_set_maxeval(sub, g_local_maxeval);
     }
     struct Cleanup {
@@ -1574,7 +1670,14 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
                 nlopt_algorithm_to_string(sub->algorithm));
         return NLOPT_INVALID_ARGS;
     }
-    if (opt->has_dx) nlopt_set_initial_step(sub, opt->dx.data());
+    if (own_sub && opt->has_xtol_abs) {            /* device options go device to device */
+        if (!opt->xtol_abs_dev.dev) nlopt_set_xtol_abs(sub, opt->xtol_abs.data());
+        else if (!copy_device_option(opt, opt->xtol_abs_dev, sub->xtol_abs_dev, sub->has_xtol_abs)) return NLOPT_FAILURE;
+    }
+    if (opt->has_dx) {
+        if (!opt->dx_dev.dev) nlopt_set_initial_step(sub, opt->dx.data());
+        else if (!copy_device_option(opt, opt->dx_dev, sub->dx_dev, sub->has_dx)) return NLOPT_FAILURE;
+    }
     opt->force_stop_child = sub;
 
     const bool sub_has_fc = alg == NLOPT_AUGLAG_EQ || alg == NLOPT_LN_AUGLAG_EQ || alg == NLOPT_LD_AUGLAG_EQ;
@@ -1664,8 +1767,10 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
         vc.ub = opt->ub.data();
         vc.x0_host = x;
         vc.x_dev = x_dev;
-        vc.x_weights = opt->has_x_weights ? opt->x_weights.data() : nullptr;
-        vc.xtol_abs = opt->has_xtol_abs ? opt->xtol_abs.data() : nullptr;
+        vc.x_weights = opt->has_x_weights && !opt->x_weights_dev.dev ? opt->x_weights.data() : nullptr;
+        vc.xtol_abs = opt->has_xtol_abs && !opt->xtol_abs_dev.dev ? opt->xtol_abs.data() : nullptr;
+        vc.x_weights_dev = opt->x_weights_dev.dev ? opt->x_weights_dev.dev->data() : nullptr;
+        vc.xtol_abs_dev = opt->xtol_abs_dev.dev ? opt->xtol_abs_dev.dev->data() : nullptr;
         vc.stats = &ev_stats;
         std::string err;
         ev.reset(nb200::make_backend(vc, &err));
@@ -1674,7 +1779,8 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
             set_err(opt, "NLOPT_AUGLAG* with device callbacks or device x runs on one GPU in this library");
             return NLOPT_INVALID_ARGS;
         }
-    }
+    } else if (!host_option(opt, opt->x_weights_dev, opt->x_weights) || !host_option(opt, opt->xtol_abs_dev, opt->xtol_abs))
+        return NLOPT_FAILURE;                        /* stop_x_host reads device options through their host mirrors */
 
     const double t_start = nb200::wall_seconds();
     auto forced = [&] { return opt->force_stop != 0; };

@@ -34,6 +34,14 @@ struct NamedParam {
     double val;
 };
 
+// device mode of one per-variable option (nlopt_b200_set_{xtol_abs,x_weights,initial_step}_device): its values live in
+// dev (owned) and the option's host vector holds them only while mirror (after a host reader downloaded them); any host
+// setter of that option frees dev
+struct DeviceOption {
+    DeviceVector *dev = nullptr;
+    bool mirror = false;
+};
+
 }  // namespace nb200
 
 struct nlopt_opt_s {
@@ -67,6 +75,7 @@ struct nlopt_opt_s {
     double ftol_rel = 0, ftol_abs = 0, xtol_rel = 0;
     bool has_xtol_abs = false, has_x_weights = false, has_dx = false;
     std::vector<double> xtol_abs, x_weights, dx;
+    nb200::DeviceOption xtol_abs_dev, x_weights_dev, dx_dev;     // has_* stays true in device mode
     int maxeval = 0, numevals = 0;
     double maxtime = 0;
     int force_stop = 0;
