@@ -1259,7 +1259,8 @@ constexpr int kTraceGens = 512;
 // mma.c:59-137), restated for one warp: lane i < m owns y_i, g_i, sigma_i, ...; the scalars are replicated in every
 // lane and every lane executes the same scalar control flow.  Sums over i are taken in index order through shuffles,
 // so every operation and its order are those of the host machine: the two produce the same bits
-// (tests/test_gpu_parity.py::test_fused_solve_equals_host_driven).
+// (tests/test_dual_machine_gpu.py replays the reference's dual trajectories into both; test_gpu_parity.py::
+// test_fused_solve_stop_rules_equal_host_driven compares whole runs).
 // MAXM bounds m at compile time: the index-order sums over the multipliers are unrolled to MAXM trips with a predicate
 // i < m, so that their shuffles are issued back to back instead of one per loop trip (they sit on the serial path of
 // every generation).
@@ -1462,8 +1463,10 @@ __device__ __noinline__ void solve_folder(const SolveArgs &sa, double *s_vs, dou
         const double y0 = lane < a.m ? a.y[lane] : 0.0, lo = lane < a.m ? sa.lo[lane] : 0.0, hi = lane < a.m ? sa.hi[lane] : 0.0;
         const int rc = mach.start(a.m, y0, lo, hi, sa.stop, lane);       // d.y carries the warm start
         if (rc != kRetSuccess) {          // start point outside the box: report, publish nothing
-            if (lane == 0) {
+            if (lane == 0) {              // the whole count record: no evaluation, no generation
+                sa.res_host[kResCounts] = 0.0;
                 sa.res_host[kResCounts + 1] = (double) rc;
+                sa.res_host[kResCounts + 2] = 0.0;
                 __threadfence_system();
                 *a.flag_host = a.seq;
                 __threadfence_system();

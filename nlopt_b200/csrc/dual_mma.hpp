@@ -12,7 +12,8 @@
 // or with a result code.  This is the HOST form (any m; DualMMA::solve drives it, one kernel launch per
 // evaluation).  The persistent dual-solve kernel carries the same algorithm as a warp-parallel,
 // register-resident machine (WarpDualMachine, ccsa_kernels.cuh: lane i owns multiplier i) that performs the
-// same IEEE operations in the same order -- tests/test_gpu_parity.py asserts bit-identical solves.
+// same IEEE operations in the same order.  Both are replayed on the reference's own trajectories, bit for bit:
+// tests/test_dual_machine.py (this file) and tests/test_dual_machine_gpu.py (the warp form).
 //   DualMachine::feed  = mma.c:145-452 specialised to "no constraints, always feasible"
 //   DualMachine::step  = mma.c:59-137 with m = 0 (the level-3 evaluation)
 #pragma once
