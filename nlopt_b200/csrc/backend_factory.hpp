@@ -12,13 +12,15 @@
 
 namespace nb200 {
 
-// one user function: exactly one of f / mf / df is set
+// One user function: the objective or one constraint object of m rows, as registered.  At most one callback pointer is
+// set, and which one is its kind: f / mf a host function, df a synchronous device callback, df2 / dmf2 / dtf an
+// asynchronous one (finished by dfin or dmfin), sf a sharded host callback.
 struct FuncSpec {
     unsigned m = 1;
     nlopt_func f = nullptr;
     nlopt_mfunc mf = nullptr;
     nlopt_b200_dfunc df = nullptr;
-    nlopt_b200_dfunc2 df2 = nullptr;         // asynchronous device callback (takes precedence over df) ...
+    nlopt_b200_dfunc2 df2 = nullptr;         // asynchronous device callback ...
     nlopt_b200_dfinish dfin = nullptr;       // ... and its host-side finish
     nlopt_b200_dmfunc2 dmf2 = nullptr;       // vector asynchronous device callback, m rows (constraints only) ...
     nlopt_b200_dmfinish dmfin = nullptr;     // ... and its host-side finish of the m totals
@@ -26,10 +28,14 @@ struct FuncSpec {
                                              // dmfin for the vector form
     int halo = 0;
     nlopt_b200_sfunc sf = nullptr;           // sharded host callback
+    nlopt_precond pre = nullptr;             // preconditioner of a host function (CCSAQ; the AUGLAG sub-problem has none)
     void *data = nullptr;
     bool negate = false;                     // objective of a maximisation (device / sharded callbacks only): the
                                              // backend minimises -f -- final value and gradient change sign
 
+    bool empty() const { return !host() && !df && !async_device() && !sharded(); }
+    bool host() const { return f || mf; }
+    bool sharded() const { return sf != nullptr; }
     // an asynchronous device callback: enqueued on the library stream, its value settled by finish_evals()
     bool async_device() const { return df2 || dmf2 || dtf; }
 };

@@ -421,33 +421,31 @@ bool DeviceBackend::setup(const BackendConfig &cfg)
     geo_.n = cfg.n;
     m_ = 0;
     max_cdim_ = 1;
+    pen_total_ = 0;
+    terms_rows_ = 0;
+    bool any_host_cb = false, any_sharded_cb = false;
+    auto scan = [&](const FuncSpec &c) {            // one walk over every function of the run
+        any_host_cb = any_host_cb || c.host();
+        any_sharded_cb = any_sharded_cb || c.sharded();
+        if (c.dtf && c.m > terms_rows_) terms_rows_ = c.m;
+    };
+    scan(cfg.objective);
     for (const FuncSpec &c : cfg.constraints) {
+        scan(c);
         m_ += c.m;
         if (c.m > max_cdim_) max_cdim_ = c.m;
     }
-    pen_total_ = 0;
     if (cfg.penalty)
         for (int pass = 0; pass < 2; ++pass)
             for (const FuncSpec &c : (pass == 0 ? cfg.penalty->eq : cfg.penalty->ineq)) {
+                scan(c);
                 pen_total_ += c.m;
                 if (c.m > max_cdim_) max_cdim_ = c.m;
             }
-    terms_rows_ = cfg.objective.dtf ? 1 : 0;
-    auto terms_rows_of = [this](const std::vector<FuncSpec> &list) {
-        for (const FuncSpec &c : list)
-            if (c.dtf && c.m > terms_rows_) terms_rows_ = c.m;
-    };
-    terms_rows_of(cfg.constraints);
-    if (cfg.penalty) {
-        terms_rows_of(cfg.penalty->eq);
-        terms_rows_of(cfg.penalty->ineq);
-    }
     if (cfg.stats) stats_ = cfg.stats;
     if (!alloc_state()) return false;
     const size_t nl = geo_.n_local, j0 = geo_.j0;
     if (cfg.values_only) {
-        bool any_host_cb = cfg.objective.f != nullptr;
-        for (const FuncSpec &c : cfg.constraints) any_host_cb = any_host_cb || c.f || c.mf;
         if (any_host_cb) NB_CUDA(cached_host_alloc(&h_x_, (size_t) geo_.n * sizeof(double)));
         if (cfg.x0_host) {
             NB_CUDA(cudaMemcpyAsync(x_, cfg.x0_host + j0, nl * sizeof(double), cudaMemcpyHostToDevice, stream_));
@@ -488,13 +486,6 @@ bool DeviceBackend::setup(const BackendConfig &cfg)
         ub_u_ = scalar_bounds_ ? cfg.ub[0] : 0.0;
     }
     sidx_valid_ = false;
-    bool any_host_cb = cfg.objective.f != nullptr;
-    for (const FuncSpec &c : cfg.constraints) any_host_cb = any_host_cb || c.f || c.mf;
-    if (cfg.penalty)
-        for (int pass = 0; pass < 2; ++pass)
-            for (const FuncSpec &c : (pass == 0 ? cfg.penalty->eq : cfg.penalty->ineq)) any_host_cb = any_host_cb || c.f || c.mf;
-    bool any_sharded_cb = cfg.objective.sf != nullptr;
-    for (const FuncSpec &c : cfg.constraints) any_sharded_cb = any_sharded_cb || c.sf;
     if (any_sharded_cb) {
         const size_t cap = geo_.n_local ? geo_.n_local : 1;
         NB_CUDA(cached_host_alloc(&h_xs_, cap * sizeof(double)));
@@ -708,12 +699,6 @@ bool DeviceBackend::host_x_for(Slot slot)
     return true;
 }
 
-bool DeviceBackend::push_grad_rows(Slot slot, int row0, unsigned rows, bool is_objective, const double *host_grad)
-{
-    double *dst = is_objective ? (slot == kBase ? g_ : gcur_) : (slot == kBase ? G_ : Gcur_) + (size_t) row0 * geo_.ld;
-    return push_rows_to(dst, rows, host_grad);
-}
-
 bool DeviceBackend::eval_objective(Slot slot, bool want_grad, double *value)
 {
     return cfg_.penalty ? eval_penalty_objective(slot, want_grad, value) : eval_user_objective(slot, want_grad, value);
@@ -744,7 +729,6 @@ bool DeviceBackend::eval_penalty_objective(Slot slot, bool want_grad, double *va
     *value = L;
     if (ps.force_stop && *ps.force_stop) return true;               // auglag.c:39
     std::vector<double> vals(pen_total_ ? pen_total_ : 1);
-    double *xs = slot == kBase ? x_ : xcur_view();
     Comm &comm = Comm::instance();
     std::vector<char> partial(pen_total_ ? pen_total_ : 1, 0);
     unsigned row = 0;
@@ -753,19 +737,11 @@ bool DeviceBackend::eval_penalty_objective(Slot slot, bool want_grad, double *va
         for (const FuncSpec &fs : (pass == 0 ? ps.eq : ps.ineq)) {
             if (fs.async_device()) {
                 for (unsigned r = 0; r < fs.m; ++r) vals[row + r] = settled[m_ + row + r];
-            } else if (fs.df) {
-                const double t0 = wall_seconds();
-                vals[row] = fs.df((unsigned) geo_.n_local, geo_.j0, xs, want_grad ? pen_rows_ + (size_t) row * geo_.ld : nullptr, fs.data, stream_);
-                cb_seconds_ += wall_seconds() - t0;
-                if (comm.active()) { partial[row] = 1; any_partial = true; }
             } else {
-                if (!host_x_for(slot)) return false;
-                double *grad = want_grad ? staging(fs.m) : nullptr;
-                const double t0 = wall_seconds();
-                if (fs.f) vals[row] = fs.f((unsigned) geo_.n, h_x_view_, grad, fs.data);        // nlopt_eval_constraint, stop.c:178-184
-                else fs.mf(fs.m, &vals[row], (unsigned) geo_.n, h_x_view_, grad, fs.data);
-                cb_seconds_ += wall_seconds() - t0;
-                if (want_grad && !push_rows_to(pen_rows_ + (size_t) row * geo_.ld, fs.m, grad)) return false;
+                bool shard_local;
+                if (!eval_fn(fs, slot, want_grad ? pen_rows_ + (size_t) row * geo_.ld : nullptr, 1 + m_ + row, &vals[row], &shard_local))
+                    return false;
+                if (shard_local) { partial[row] = 1; any_partial = true; }
             }
             row += fs.m;
             if (ps.force_stop && *ps.force_stop) return true;
@@ -843,86 +819,76 @@ bool DeviceBackend::negate_gradient(double *g)
     return true;
 }
 
+// One user function of any kind at the slot.  Its values go to values[0, m): those of an asynchronous callback read 0
+// here and are settled by finish_evals() from the value slots [index, index + m).  Its gradient rows go to grad_dst,
+// stride ld (null: no gradient).  *shard_local: values[0] is this rank's share of a sum over the ranks (a synchronous
+// device or a sharded callback on several ranks), which the caller settles.
+bool DeviceBackend::eval_fn(const FuncSpec &fs, Slot slot, double *grad_dst, unsigned index, double *values, bool *shard_local)
+{
+    *shard_local = false;
+    if (fs.sharded()) {
+        if (!eval_sharded(fs, slot, grad_dst, values)) return false;
+        *shard_local = Comm::instance().active();
+        return true;
+    }
+    if (fs.async_device()) {
+        for (unsigned r = 0; r < fs.m; ++r) values[r] = 0.0;
+        return enqueue_df2(fs, slot, grad_dst, index);
+    }
+    if (fs.df) {
+        double *xs = slot == kBase ? x_ : xcur_view();
+        const double t0 = wall_seconds();
+        values[0] = fs.df((unsigned) geo_.n_local, geo_.j0, xs, grad_dst, fs.data, stream_);
+        cb_seconds_ += wall_seconds() - t0;
+        *shard_local = Comm::instance().active();
+        return true;
+    }
+    if (!host_x_for(slot)) return false;       // usually a no-op: an earlier callback of the point mirrored x already
+    double *grad = grad_dst ? staging(fs.m) : nullptr;
+    const double t0 = wall_seconds();
+    if (fs.f) values[0] = fs.f((unsigned) geo_.n, h_x_view_, grad, fs.data);        // nlopt_eval_constraint, stop.c:178-184
+    else fs.mf(fs.m, values, (unsigned) geo_.n, h_x_view_, grad, fs.data);
+    cb_seconds_ += wall_seconds() - t0;
+    return !grad_dst || push_rows_to(grad_dst, fs.m, grad);
+}
+
 // With FuncSpec::negate the objective's value changes sign once it is final: here for one rank, in finish_evals() for
 // shard contributions and for the asynchronous form.
 bool DeviceBackend::eval_user_objective(Slot slot, bool want_grad, double *value)
 {
     const FuncSpec &fs = cfg_.objective;
-    if (fs.sf) {
-        double *gs = want_grad ? (slot == kBase ? g_ : gcur_) : nullptr;
-        if (!eval_sharded(fs, slot, gs, 0, value)) return false;
-        if (fs.negate && !Comm::instance().active()) *value = -*value;
-        return !fs.negate || negate_gradient(gs);
+    if (fs.empty()) return fail("no objective function");
+    double *gs = want_grad ? (slot == kBase ? g_ : gcur_) : nullptr;
+    bool shard_local;
+    if (!eval_fn(fs, slot, gs, 0, value, &shard_local)) return false;
+    if (shard_local) {                             // shard contributions add up: settled in finish_evals()
+        pend_val_[0] = *value;
+        pend_set_[0] = 1;
+        pend_any_ = true;
     }
-    if (fs.async_device()) {
-        double *gs = want_grad ? (slot == kBase ? g_ : gcur_) : nullptr;
-        *value = 0.0;                                  // settled in finish_evals()
-        if (!enqueue_df2(fs, slot, gs, 0)) return false;
-        return !fs.negate || negate_gradient(gs);
-    }
-    if (fs.df) {
-        double *xs = slot == kBase ? x_ : xcur_view();
-        double *gs = want_grad ? (slot == kBase ? g_ : gcur_) : nullptr;
-        const double t0 = wall_seconds();
-        double v = fs.df((unsigned) geo_.n_local, geo_.j0, xs, gs, fs.data, stream_);
-        cb_seconds_ += wall_seconds() - t0;
-        if (Comm::instance().active()) {           // shard contributions add up: settled in finish_evals()
-            pend_val_[0] = v;
-            pend_set_[0] = 1;
-            pend_any_ = true;
-        } else if (fs.negate)
-            v = -v;
-        *value = v;
-        return !fs.negate || negate_gradient(gs);
-    }
-    if (!fs.f) return fail("no objective function");
-    if (!host_x_for(slot)) return false;
-    double *grad = want_grad ? staging(1) : nullptr;
-    const double t0 = wall_seconds();
-    *value = fs.f((unsigned) geo_.n, h_x_view_, grad, fs.data);
-    cb_seconds_ += wall_seconds() - t0;
-    if (want_grad) return push_grad_rows(slot, 0, 1, true, grad);
-    return true;
+    if (!fs.negate) return true;
+    if (!shard_local && !fs.async_device()) *value = -*value;
+    return negate_gradient(gs);
 }
 
 bool DeviceBackend::eval_constraint(Slot slot, unsigned ic, unsigned row0, bool want_grad, double *values)
 {
-    const FuncSpec &fs = cfg_.constraints[ic];
-    if (fs.sf) return eval_sharded(fs, slot, want_grad ? (slot == kBase ? G_ : Gcur_) + (size_t) row0 * geo_.ld : nullptr, 1 + row0, values);
-    if (fs.async_device()) {
-        double *gs = want_grad ? (slot == kBase ? G_ : Gcur_) + (size_t) row0 * geo_.ld : nullptr;
-        for (unsigned r = 0; r < fs.m; ++r) values[r] = 0.0;
-        return enqueue_df2(fs, slot, gs, 1 + row0);
+    double *gs = want_grad ? (slot == kBase ? G_ : Gcur_) + (size_t) row0 * geo_.ld : nullptr;
+    bool shard_local;
+    if (!eval_fn(cfg_.constraints[ic], slot, gs, 1 + row0, values, &shard_local)) return false;
+    if (shard_local) {
+        pend_val_[1 + row0] = values[0];
+        pend_set_[1 + row0] = 1;
+        pend_any_ = true;
     }
-    if (fs.df) {
-        double *xs = slot == kBase ? x_ : xcur_view();
-        double *gs = want_grad ? (slot == kBase ? G_ : Gcur_) + (size_t) row0 * geo_.ld : nullptr;
-        const double t0 = wall_seconds();
-        double v = fs.df((unsigned) geo_.n_local, geo_.j0, xs, gs, fs.data, stream_);
-        cb_seconds_ += wall_seconds() - t0;
-        if (Comm::instance().active()) {
-            pend_val_[1 + row0] = v;
-            pend_set_[1 + row0] = 1;
-            pend_any_ = true;
-        }
-        values[0] = v;
-        return true;
-    }
-    if (!host_x_for(slot)) return false;       // usually a no-op: the objective call mirrored x already
-    double *grad = want_grad ? staging(fs.m) : nullptr;
-    const double t0 = wall_seconds();
-    if (fs.f) values[0] = fs.f((unsigned) geo_.n, h_x_view_, grad, fs.data);        // nlopt_eval_constraint, stop.c:178-184
-    else fs.mf(fs.m, values, (unsigned) geo_.n, h_x_view_, grad, fs.data);
-    cb_seconds_ += wall_seconds() - t0;
-    if (want_grad) return push_grad_rows(slot, (int) row0, fs.m, false, grad);
     return true;
 }
 
-// Device callbacks on several ranks return shard-local values; one all-reduce settles every value of the point
-// (1 + m doubles; entries from host callbacks are global already and are not touched).
+// Device callbacks on several ranks return shard-local values; one all-reduce in finish_evals() settles every value of
+// the point (1 + m doubles; entries from host callbacks are global already and are not touched).
 // Sharded host callbacks (nlopt_b200_sfunc): this rank's n_local variables down, its n_local gradient entries up, the
-// additive value contribution settled with the others in finish_evals().
-bool DeviceBackend::eval_sharded(const FuncSpec &fs, Slot slot, double *grad_dst, unsigned index, double *value)
+// value this rank's additive contribution.
+bool DeviceBackend::eval_sharded(const FuncSpec &fs, Slot slot, double *grad_dst, double *value)
 {
     const size_t nl = geo_.n_local;
     const double *src = slot == kBase ? x_ : xcur_view();
@@ -942,7 +908,7 @@ bool DeviceBackend::eval_sharded(const FuncSpec &fs, Slot slot, double *grad_dst
         grad = h_gs_[b];
     }
     const double t0 = wall_seconds();
-    const double v = fs.sf((unsigned) nl, geo_.j0, geo_.n, h_xs_, grad, fs.data);
+    *value = fs.sf((unsigned) nl, geo_.j0, geo_.n, h_xs_, grad, fs.data);
     cb_seconds_ += wall_seconds() - t0;
     if (grad_dst) {
         NB_CUDA(cudaMemcpyAsync(grad_dst, grad, nl * sizeof(double), cudaMemcpyHostToDevice, copy_stream_));
@@ -950,12 +916,6 @@ bool DeviceBackend::eval_sharded(const FuncSpec &fs, Slot slot, double *grad_dst
         NB_CUDA(cudaStreamWaitEvent(stream_, h_gs_done_[b], 0));
         stats_->h2d_bytes += nl * sizeof(double);
     }
-    if (Comm::instance().active()) {
-        pend_val_[index] = v;
-        pend_set_[index] = 1;
-        pend_any_ = true;
-    }
-    *value = v;
     return true;
 }
 

@@ -42,7 +42,7 @@ public:
     bool enqueue_df2(const FuncSpec &fs, Slot slot, double *grad_dst, unsigned index);
     bool reduce_terms(const FuncSpec &fs, const double *xs, double *grad_dst, double *vsums);
     bool ensure_halo(Slot slot);
-    bool eval_sharded(const FuncSpec &fs, Slot slot, double *grad_dst, unsigned index, double *value);
+    bool eval_sharded(const FuncSpec &fs, Slot slot, double *grad_dst, double *value);
     bool eval_user_objective(Slot slot, bool want_grad, double *value);
     bool negate_gradient(double *g);
     bool push_rows_to(double *dst, unsigned rows, const double *host_grad);
@@ -94,7 +94,7 @@ private:
     bool sigma_index_runs() const;
     bool wait_flag();
     bool host_x_for(Slot slot);                      // bring the slot's x to pinned host memory (cached per epoch)
-    bool push_grad_rows(Slot slot, int row0, unsigned rows, bool is_objective, const double *host_grad);
+    bool eval_fn(const FuncSpec &fs, Slot slot, double *grad_dst, unsigned index, double *values, bool *shard_local);
     double *staging(unsigned rows);
     struct Owned { void *p; size_t bytes; bool pinned; };
     std::vector<Owned> owned_;                       // small buffers borrowed from the block cache

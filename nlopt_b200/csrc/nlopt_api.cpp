@@ -17,6 +17,7 @@
 #include "nlopt_object.hpp"
 
 using nb200::ConstraintRec;
+using nb200::FuncSpec;
 using nb200::NamedParam;
 
 namespace {
@@ -170,26 +171,54 @@ bool equality_ok(nlopt_algorithm a)
 void munge_all(nlopt_opt o, std::vector<ConstraintRec> &v)
 {
     if (o->munge_on_destroy)
-        for (auto &c : v) o->munge_on_destroy(c.f_data);
+        for (auto &c : v) o->munge_on_destroy(c.fn.data);
 }
 
 // options.c:504-547
-// vector_form: dfc is the marker of a vector device callback (nlopt_b200_add_*_mconstraint_device2), any fm
-nlopt_result add_constraint(nlopt_opt opt, std::vector<ConstraintRec> &list, unsigned fm, nlopt_func fc,
-                            nlopt_mfunc mfc, nlopt_b200_dfunc dfc, nlopt_precond pre, void *data, const double *tol,
-                            bool vector_form)
+nlopt_result add_constraint(nlopt_opt opt, std::vector<ConstraintRec> &list, const FuncSpec &fn, const double *tol)
 {
-    const int kinds = (fc != nullptr) + (mfc != nullptr) + (dfc != nullptr);
-    if (kinds != 1 || ((fc || (dfc && !vector_form)) && fm != 1)) return NLOPT_INVALID_ARGS;
+    if (fn.empty()) return NLOPT_INVALID_ARGS;
     if (tol)
-        for (unsigned i = 0; i < fm; ++i)
+        for (unsigned i = 0; i < fn.m; ++i)
             if (tol[i] < 0) { set_err(opt, "negative constraint tolerance"); return NLOPT_INVALID_ARGS; }
-    ConstraintRec r;
-    r.m = fm; r.f = fc; r.mf = mfc; r.df = dfc; r.pre = pre; r.f_data = data;
-    r.tol.assign(fm, 0.0);
-    if (tol) r.tol.assign(tol, tol + fm);
+    ConstraintRec r{fn, std::vector<double>(fn.m, 0.0)};
+    if (tol) r.tol.assign(tol, tol + fn.m);
     try { list.push_back(r); } catch (const std::bad_alloc &) { return NLOPT_OUT_OF_MEMORY; }
     return NLOPT_SUCCESS;
+}
+
+// the record of each registration form
+FuncSpec host_spec(nlopt_func f, nlopt_precond pre, void *data) { FuncSpec s; s.f = f; s.pre = pre; s.data = data; return s; }
+FuncSpec host_mspec(unsigned m, nlopt_mfunc mf, void *data) { FuncSpec s; s.m = m; s.mf = mf; s.data = data; return s; }
+FuncSpec device_spec(nlopt_b200_dfunc df, void *data) { FuncSpec s; s.df = df; s.data = data; return s; }
+FuncSpec sharded_spec(nlopt_b200_sfunc sf, void *data) { FuncSpec s; s.sf = sf; s.data = data; return s; }
+FuncSpec device2_spec(unsigned m, nlopt_b200_dfunc2 f, nlopt_b200_dmfunc2 mf, nlopt_b200_dfinish fin, nlopt_b200_dmfinish mfin,
+                      void *data, int halo)
+{
+    FuncSpec s;
+    s.m = m; s.df2 = f; s.dmf2 = mf; s.dfin = fin; s.dmfin = mfin; s.data = data; s.halo = halo;
+    return s;
+}
+// per-variable terms: a scalar function finishes in dfin, m rows in dmfin
+FuncSpec terms_spec(unsigned m, nlopt_b200_dtfunc f, nlopt_b200_dfinish fin, nlopt_b200_dmfinish mfin, void *data, int halo)
+{
+    FuncSpec s;
+    s.m = m; s.dtf = f; s.dfin = fin; s.dmfin = mfin; s.data = data; s.halo = halo;
+    return s;
+}
+
+// The argument checks of the asynchronous forms (a callback, its finish, halo 0 or 1) and of the sharded form (a
+// callback).  Their entry points make them before anything else: a refusal leaves the error message and the data alone.
+bool complete(const FuncSpec &s)
+{
+    return s.sharded() || (s.async_device() && (s.dfin || s.dmfin) && (s.halo == 0 || s.halo == 1));
+}
+
+// nlopt_eval_constraint (stop.c:178-184) of a host function
+void eval_host(const FuncSpec &c, unsigned n, const double *x, double *out, double *grad)
+{
+    if (c.f) out[0] = c.f(n, x, grad, c.data);
+    else c.mf(c.m, out, n, x, grad, c.data);
 }
 
 struct AlgInfo { const char *id; const char *desc; };
@@ -339,7 +368,7 @@ void nlopt_destroy(nlopt_opt opt)
 {
     if (!opt) return;
     if (opt->munge_on_destroy) {
-        opt->munge_on_destroy(opt->f_data);
+        opt->munge_on_destroy(opt->objective.data);
         munge_all(opt, opt->fc);
         munge_all(opt, opt->h);
     }
@@ -374,9 +403,9 @@ nlopt_opt nlopt_copy(const nlopt_opt opt)
     }
     if (nlopt_munge mg = c->munge_on_copy) {
         bool bad = false;
-        if (c->f_data && !(c->f_data = mg(c->f_data))) bad = true;
-        for (auto &r : c->fc) if (!bad && r.f_data && !(r.f_data = mg(r.f_data))) bad = true;
-        for (auto &r : c->h) if (!bad && r.f_data && !(r.f_data = mg(r.f_data))) bad = true;
+        if (c->objective.data && !(c->objective.data = mg(c->objective.data))) bad = true;
+        for (auto &r : c->fc) if (!bad && r.fn.data && !(r.fn.data = mg(r.fn.data))) bad = true;
+        for (auto &r : c->h) if (!bad && r.fn.data && !(r.fn.data = mg(r.fn.data))) bad = true;
         if (bad) {                       /* options.c:261-263: better to leak than to crash */
             c->munge_on_destroy = nullptr;
             nlopt_destroy(c);
@@ -393,21 +422,12 @@ nlopt_opt nlopt_copy(const nlopt_opt opt)
 
 /* ------------------------------------------------------------------ objective (options.c:322-364) */
 
-static nlopt_result set_objective(nlopt_opt opt, nlopt_func f, nlopt_b200_dfunc df, nlopt_precond pre, void *data,
-                                  int maximize)
+static nlopt_result set_objective(nlopt_opt opt, const FuncSpec &fn, int maximize)
 {
     if (!opt) return NLOPT_INVALID_ARGS;
     clear_err(opt);
-    if (opt->munge_on_destroy) opt->munge_on_destroy(opt->f_data);
-    opt->f = f;
-    opt->df = df;
-    opt->df2 = nullptr;
-    opt->dfin = nullptr;
-    opt->dtf = nullptr;
-    opt->halo = 0;
-    opt->sf = nullptr;
-    opt->f_data = data;
-    opt->pre = pre;
+    if (opt->munge_on_destroy) opt->munge_on_destroy(opt->objective.data);
+    opt->objective = fn;
     opt->maximize = maximize;
     if (nb200::nl_isinf(opt->stopval)) {
         if (!maximize && opt->stopval > 0) opt->stopval = -kInf;
@@ -415,67 +435,33 @@ static nlopt_result set_objective(nlopt_opt opt, nlopt_func f, nlopt_b200_dfunc 
     }
     return NLOPT_SUCCESS;
 }
+static nlopt_result set_objective_checked(nlopt_opt opt, const FuncSpec &fn, int maximize)
+{ return complete(fn) ? set_objective(opt, fn, maximize) : NLOPT_INVALID_ARGS; }
 
 nlopt_result nlopt_set_precond_min_objective(nlopt_opt opt, nlopt_func f, nlopt_precond pre, void *d)
-{ return set_objective(opt, f, nullptr, pre, d, 0); }
+{ return set_objective(opt, host_spec(f, pre, d), 0); }
 nlopt_result nlopt_set_min_objective(nlopt_opt opt, nlopt_func f, void *d)
-{ return set_objective(opt, f, nullptr, nullptr, d, 0); }
+{ return set_objective(opt, host_spec(f, nullptr, d), 0); }
 nlopt_result nlopt_set_precond_max_objective(nlopt_opt opt, nlopt_func f, nlopt_precond pre, void *d)
-{ return set_objective(opt, f, nullptr, pre, d, 1); }
+{ return set_objective(opt, host_spec(f, pre, d), 1); }
 nlopt_result nlopt_set_max_objective(nlopt_opt opt, nlopt_func f, void *d)
-{ return set_objective(opt, f, nullptr, nullptr, d, 1); }
+{ return set_objective(opt, host_spec(f, nullptr, d), 1); }
 nlopt_result nlopt_b200_set_min_objective_device(nlopt_opt opt, nlopt_b200_dfunc f, void *d)
-{ return set_objective(opt, nullptr, f, nullptr, d, 0); }
+{ return set_objective(opt, device_spec(f, d), 0); }
 nlopt_result nlopt_b200_set_max_objective_device(nlopt_opt opt, nlopt_b200_dfunc f, void *d)
-{ return set_objective(opt, nullptr, f, nullptr, d, 1); }
-
-/* marker stored in the `df` field of callbacks registered in the asynchronous form: never called */
-static double df2_marker(unsigned, unsigned long long, const double *, double *, void *, void *) { return 0.0; }
-
-static nlopt_result set_objective_device2(nlopt_opt opt, nlopt_b200_dfunc2 f, nlopt_b200_dfinish fin, void *d, int halo,
-                                          int maximize)
-{
-    if (!f || !fin || halo < 0 || halo > 1) return NLOPT_INVALID_ARGS;
-    nlopt_result r = set_objective(opt, nullptr, df2_marker, nullptr, d, maximize);
-    if (r < 0) return r;
-    opt->df2 = f;
-    opt->dfin = fin;
-    opt->halo = halo;
-    return r;
-}
+{ return set_objective(opt, device_spec(f, d), 1); }
 nlopt_result nlopt_b200_set_min_objective_device2(nlopt_opt opt, nlopt_b200_dfunc2 f, nlopt_b200_dfinish fin, void *d, int halo)
-{ return set_objective_device2(opt, f, fin, d, halo, 0); }
+{ return set_objective_checked(opt, device2_spec(1, f, nullptr, fin, nullptr, d, halo), 0); }
 nlopt_result nlopt_b200_set_max_objective_device2(nlopt_opt opt, nlopt_b200_dfunc2 f, nlopt_b200_dfinish fin, void *d, int halo)
-{ return set_objective_device2(opt, f, fin, d, halo, 1); }
-
-static nlopt_result set_objective_terms(nlopt_opt opt, nlopt_b200_dtfunc f, nlopt_b200_dfinish fin, void *d, int halo,
-                                        int maximize)
-{
-    if (!f || !fin || halo < 0 || halo > 1) return NLOPT_INVALID_ARGS;
-    nlopt_result r = set_objective(opt, nullptr, df2_marker, nullptr, d, maximize);
-    if (r < 0) return r;
-    opt->dtf = f;
-    opt->dfin = fin;
-    opt->halo = halo;
-    return r;
-}
+{ return set_objective_checked(opt, device2_spec(1, f, nullptr, fin, nullptr, d, halo), 1); }
 nlopt_result nlopt_b200_set_min_objective_terms(nlopt_opt opt, nlopt_b200_dtfunc f, nlopt_b200_dfinish fin, void *d, int halo)
-{ return set_objective_terms(opt, f, fin, d, halo, 0); }
+{ return set_objective_checked(opt, terms_spec(1, f, fin, nullptr, d, halo), 0); }
 nlopt_result nlopt_b200_set_max_objective_terms(nlopt_opt opt, nlopt_b200_dtfunc f, nlopt_b200_dfinish fin, void *d, int halo)
-{ return set_objective_terms(opt, f, fin, d, halo, 1); }
-
-static nlopt_result set_objective_sharded(nlopt_opt opt, nlopt_b200_sfunc f, void *d, int maximize)
-{
-    if (!f) return NLOPT_INVALID_ARGS;
-    nlopt_result r = set_objective(opt, nullptr, df2_marker, nullptr, d, maximize);
-    if (r < 0) return r;
-    opt->sf = f;
-    return r;
-}
+{ return set_objective_checked(opt, terms_spec(1, f, fin, nullptr, d, halo), 1); }
 nlopt_result nlopt_b200_set_min_objective_sharded(nlopt_opt opt, nlopt_b200_sfunc f, void *d)
-{ return set_objective_sharded(opt, f, d, 0); }
+{ return set_objective_checked(opt, sharded_spec(f, d), 0); }
 nlopt_result nlopt_b200_set_max_objective_sharded(nlopt_opt opt, nlopt_b200_sfunc f, void *d)
-{ return set_objective_sharded(opt, f, d, 1); }
+{ return set_objective_checked(opt, sharded_spec(f, d), 1); }
 
 nlopt_algorithm nlopt_get_algorithm(const nlopt_opt opt) { return opt->algorithm; }
 unsigned nlopt_get_dimension(const nlopt_opt opt) { return opt->n; }
@@ -627,13 +613,12 @@ nlopt_result nlopt_remove_equality_constraints(nlopt_opt opt)
     return NLOPT_SUCCESS;
 }
 
-static nlopt_result add_any(nlopt_opt opt, bool equality, bool vector_form, unsigned m, nlopt_func fc,
-                            nlopt_mfunc mfc, nlopt_b200_dfunc dfc, nlopt_precond pre, void *data, const double *tol)
+static nlopt_result add_any(nlopt_opt opt, bool equality, const FuncSpec &fn, const double *tol)
 {
     nlopt_result ret;
     clear_err(opt);
-    if (vector_form && !m) {                 /* options.c:560-564: an empty vector constraint is fine */
-        if (opt && opt->munge_on_destroy) opt->munge_on_destroy(data);
+    if (!fn.m) {                             /* options.c:560-564: an empty vector constraint is fine */
+        if (opt && opt->munge_on_destroy) opt->munge_on_destroy(fn.data);
         return NLOPT_SUCCESS;
     }
     if (!opt) ret = NLOPT_INVALID_ARGS;
@@ -641,119 +626,56 @@ static nlopt_result add_any(nlopt_opt opt, bool equality, bool vector_form, unsi
         set_err(opt, "invalid algorithm for constraints");
         ret = NLOPT_INVALID_ARGS;
     } else
-        ret = add_constraint(opt, equality ? opt->h : opt->fc, m, fc, mfc, dfc, pre, data, tol, vector_form);
-    if (ret < 0 && opt && opt->munge_on_destroy) opt->munge_on_destroy(data);
+        ret = add_constraint(opt, equality ? opt->h : opt->fc, fn, tol);
+    if (ret < 0 && opt && opt->munge_on_destroy) opt->munge_on_destroy(fn.data);
     return ret;
 }
+// the vector forms check their arguments only when m > 0 (m == 0 registers nothing)
+static nlopt_result add_checked(nlopt_opt opt, bool equality, const FuncSpec &fn, const double *tol)
+{ return !fn.m || complete(fn) ? add_any(opt, equality, fn, tol) : NLOPT_INVALID_ARGS; }
 
 nlopt_result nlopt_add_inequality_mconstraint(nlopt_opt opt, unsigned m, nlopt_mfunc fc, void *d, const double *tol)
-{ return add_any(opt, false, true, m, nullptr, fc, nullptr, nullptr, d, tol); }
+{ return add_any(opt, false, host_mspec(m, fc, d), tol); }
 nlopt_result nlopt_add_precond_inequality_constraint(nlopt_opt opt, nlopt_func fc, nlopt_precond pre, void *d, double tol)
-{ return add_any(opt, false, false, 1, fc, nullptr, nullptr, pre, d, &tol); }
+{ return add_any(opt, false, host_spec(fc, pre, d), &tol); }
 nlopt_result nlopt_add_inequality_constraint(nlopt_opt opt, nlopt_func fc, void *d, double tol)
-{ return add_any(opt, false, false, 1, fc, nullptr, nullptr, nullptr, d, &tol); }
+{ return add_any(opt, false, host_spec(fc, nullptr, d), &tol); }
 nlopt_result nlopt_b200_add_inequality_constraint_device(nlopt_opt opt, nlopt_b200_dfunc fc, void *d, double tol)
-{ return add_any(opt, false, false, 1, nullptr, nullptr, fc, nullptr, d, &tol); }
+{ return add_any(opt, false, device_spec(fc, d), &tol); }
 nlopt_result nlopt_b200_add_inequality_constraint_device2(nlopt_opt opt, nlopt_b200_dfunc2 fc, nlopt_b200_dfinish fin, void *d,
                                                           double tol, int halo)
-{
-    if (!fc || !fin || halo < 0 || halo > 1) return NLOPT_INVALID_ARGS;
-    nlopt_result r = add_any(opt, false, false, 1, nullptr, nullptr, df2_marker, nullptr, d, &tol);
-    if (r < 0) return r;
-    nb200::ConstraintRec &c = opt->fc.back();
-    c.df2 = fc;
-    c.dfin = fin;
-    c.halo = halo;
-    return r;
-}
+{ return add_checked(opt, false, device2_spec(1, fc, nullptr, fin, nullptr, d, halo), &tol); }
 nlopt_result nlopt_b200_add_inequality_constraint_sharded(nlopt_opt opt, nlopt_b200_sfunc fc, void *d, double tol)
-{
-    if (!fc) return NLOPT_INVALID_ARGS;
-    nlopt_result r = add_any(opt, false, false, 1, nullptr, nullptr, df2_marker, nullptr, d, &tol);
-    if (r < 0) return r;
-    opt->fc.back().sf = fc;
-    return r;
-}
+{ return add_checked(opt, false, sharded_spec(fc, d), &tol); }
 nlopt_result nlopt_add_equality_mconstraint(nlopt_opt opt, unsigned m, nlopt_mfunc h, void *d, const double *tol)
-{ return add_any(opt, true, true, m, nullptr, h, nullptr, nullptr, d, tol); }
+{ return add_any(opt, true, host_mspec(m, h, d), tol); }
 nlopt_result nlopt_add_precond_equality_constraint(nlopt_opt opt, nlopt_func h, nlopt_precond pre, void *d, double tol)
-{ return add_any(opt, true, false, 1, h, nullptr, nullptr, pre, d, &tol); }
+{ return add_any(opt, true, host_spec(h, pre, d), &tol); }
 nlopt_result nlopt_add_equality_constraint(nlopt_opt opt, nlopt_func h, void *d, double tol)
-{ return add_any(opt, true, false, 1, h, nullptr, nullptr, nullptr, d, &tol); }
+{ return add_any(opt, true, host_spec(h, nullptr, d), &tol); }
 nlopt_result nlopt_b200_add_equality_constraint_device(nlopt_opt opt, nlopt_b200_dfunc h, void *d, double tol)
-{ return add_any(opt, true, false, 1, nullptr, nullptr, h, nullptr, d, &tol); }
+{ return add_any(opt, true, device_spec(h, d), &tol); }
 nlopt_result nlopt_b200_add_equality_constraint_device2(nlopt_opt opt, nlopt_b200_dfunc2 h, nlopt_b200_dfinish fin, void *d,
                                                         double tol, int halo)
-{
-    if (!h || !fin || halo < 0 || halo > 1) return NLOPT_INVALID_ARGS;
-    nlopt_result r = add_any(opt, true, false, 1, nullptr, nullptr, df2_marker, nullptr, d, &tol);
-    if (r < 0) return r;
-    nb200::ConstraintRec &c = opt->h.back();
-    c.df2 = h;
-    c.dfin = fin;
-    c.halo = halo;
-    return r;
-}
-
-// the vector twins: registered like nlopt_add_*_mconstraint (m == 0 is accepted and registers nothing), with the
-// scalar _device2 argument checks and the marker in df
-static nlopt_result add_device_m(nlopt_opt opt, bool equality, unsigned m, nlopt_b200_dmfunc2 fc, nlopt_b200_dmfinish fin,
-                                 void *d, const double *tol, int halo)
-{
-    if (m && (!fc || !fin || halo < 0 || halo > 1)) return NLOPT_INVALID_ARGS;
-    nlopt_result r = add_any(opt, equality, true, m, nullptr, nullptr, df2_marker, nullptr, d, tol);
-    if (r < 0 || !m) return r;
-    nb200::ConstraintRec &c = (equality ? opt->h : opt->fc).back();
-    c.dmf2 = fc;
-    c.dmfin = fin;
-    c.halo = halo;
-    return r;
-}
+{ return add_checked(opt, true, device2_spec(1, h, nullptr, fin, nullptr, d, halo), &tol); }
 nlopt_result nlopt_b200_add_inequality_mconstraint_device2(nlopt_opt opt, unsigned m, nlopt_b200_dmfunc2 fc,
                                                            nlopt_b200_dmfinish fin, void *d, const double *tol, int halo)
-{ return add_device_m(opt, false, m, fc, fin, d, tol, halo); }
+{ return add_checked(opt, false, device2_spec(m, nullptr, fc, nullptr, fin, d, halo), tol); }
 nlopt_result nlopt_b200_add_equality_mconstraint_device2(nlopt_opt opt, unsigned m, nlopt_b200_dmfunc2 h,
                                                          nlopt_b200_dmfinish fin, void *d, const double *tol, int halo)
-{ return add_device_m(opt, true, m, h, fin, d, tol, halo); }
-
-// per-variable terms (nlopt_b200_dtfunc): the scalar forms check and register like the _device2 twins, the vector forms
-// like the _mconstraint_device2 twins; the callback goes in dtf, the finish in dfin / dmfin
-static nlopt_result add_terms(nlopt_opt opt, bool equality, nlopt_b200_dtfunc fc, nlopt_b200_dfinish fin, void *d, double tol,
-                              int halo)
-{
-    if (!fc || !fin || halo < 0 || halo > 1) return NLOPT_INVALID_ARGS;
-    nlopt_result r = add_any(opt, equality, false, 1, nullptr, nullptr, df2_marker, nullptr, d, &tol);
-    if (r < 0) return r;
-    nb200::ConstraintRec &c = (equality ? opt->h : opt->fc).back();
-    c.dtf = fc;
-    c.dfin = fin;
-    c.halo = halo;
-    return r;
-}
-static nlopt_result add_terms_m(nlopt_opt opt, bool equality, unsigned m, nlopt_b200_dtfunc fc, nlopt_b200_dmfinish fin,
-                                void *d, const double *tol, int halo)
-{
-    if (m && (!fc || !fin || halo < 0 || halo > 1)) return NLOPT_INVALID_ARGS;
-    nlopt_result r = add_any(opt, equality, true, m, nullptr, nullptr, df2_marker, nullptr, d, tol);
-    if (r < 0 || !m) return r;
-    nb200::ConstraintRec &c = (equality ? opt->h : opt->fc).back();
-    c.dtf = fc;
-    c.dmfin = fin;
-    c.halo = halo;
-    return r;
-}
+{ return add_checked(opt, true, device2_spec(m, nullptr, h, nullptr, fin, d, halo), tol); }
 nlopt_result nlopt_b200_add_inequality_constraint_terms(nlopt_opt opt, nlopt_b200_dtfunc fc, nlopt_b200_dfinish fin, void *d,
                                                         double tol, int halo)
-{ return add_terms(opt, false, fc, fin, d, tol, halo); }
+{ return add_checked(opt, false, terms_spec(1, fc, fin, nullptr, d, halo), &tol); }
 nlopt_result nlopt_b200_add_equality_constraint_terms(nlopt_opt opt, nlopt_b200_dtfunc h, nlopt_b200_dfinish fin, void *d,
                                                       double tol, int halo)
-{ return add_terms(opt, true, h, fin, d, tol, halo); }
+{ return add_checked(opt, true, terms_spec(1, h, fin, nullptr, d, halo), &tol); }
 nlopt_result nlopt_b200_add_inequality_mconstraint_terms(nlopt_opt opt, unsigned m, nlopt_b200_dtfunc fc,
                                                          nlopt_b200_dmfinish fin, void *d, const double *tol, int halo)
-{ return add_terms_m(opt, false, m, fc, fin, d, tol, halo); }
+{ return add_checked(opt, false, terms_spec(m, fc, nullptr, fin, d, halo), tol); }
 nlopt_result nlopt_b200_add_equality_mconstraint_terms(nlopt_opt opt, unsigned m, nlopt_b200_dtfunc h,
                                                        nlopt_b200_dmfinish fin, void *d, const double *tol, int halo)
-{ return add_terms_m(opt, true, m, h, fin, d, tol, halo); }
+{ return add_checked(opt, true, terms_spec(m, h, nullptr, fin, d, halo), tol); }
 
 /* ------------------------------------------------------------------ stopping criteria (options.c:661-816) */
 
@@ -967,9 +889,9 @@ void nlopt_set_munge(nlopt_opt opt, nlopt_munge on_destroy, nlopt_munge on_copy)
 void nlopt_munge_data(nlopt_opt opt, nlopt_munge2 munge, void *data)
 {
     if (!opt || !munge) return;
-    opt->f_data = munge(opt->f_data, data);
-    for (auto &c : opt->fc) c.f_data = munge(c.f_data, data);
-    for (auto &c : opt->h) c.f_data = munge(c.f_data, data);
+    opt->objective.data = munge(opt->objective.data, data);
+    for (auto &c : opt->fc) c.fn.data = munge(c.fn.data, data);
+    for (auto &c : opt->h) c.fn.data = munge(c.fn.data, data);
 }
 
 nlopt_result nlopt_b200_get_stats(const nlopt_opt opt, nlopt_b200_stats *out)
@@ -984,7 +906,7 @@ nlopt_result nlopt_b200_get_stats(const nlopt_opt opt, nlopt_b200_stats *out)
 static nlopt_result optimize_common(nlopt_opt opt, double *x_host, double *x_dev, double *opt_f)
 {
     clear_err(opt);
-    if (!opt || !opt_f || (!opt->f && !opt->df)) {
+    if (!opt || !opt_f || opt->objective.empty()) {
         set_err(opt, "NULL args to nlopt_optimize");
         return NLOPT_INVALID_ARGS;
     }
@@ -993,17 +915,18 @@ static nlopt_result optimize_common(nlopt_opt opt, double *x_host, double *x_dev
 
     /* maximisation: minimise the sign-flipped objective, then restore (optimize.c:1014-1024, :1070-1077).  A host
        objective is wrapped in flipped(); a device or sharded objective keeps its callback and the backend negates its
-       final value and its gradient (opt->negate -> FuncSpec::negate) */
-    nlopt_func f0 = opt->f;
-    void *d0 = opt->f_data;
+       final value and its gradient (FuncSpec::negate) */
+    FuncSpec &obj = opt->objective;
+    nlopt_func f0 = obj.f;
+    void *d0 = obj.data;
     FlipData flip{f0, d0};
     const int maximize = opt->maximize;
     if (maximize) {
-        if (opt->f) {
-            opt->f = flipped;
-            opt->f_data = &flip;
+        if (obj.f) {
+            obj.f = flipped;
+            obj.data = &flip;
         } else
-            opt->negate = 1;
+            obj.negate = true;
         opt->stopval = -opt->stopval;
         opt->maximize = 0;
     }
@@ -1014,10 +937,10 @@ static nlopt_result optimize_common(nlopt_opt opt, double *x_host, double *x_dev
         ret = run_ccsa(opt, x_host, x_dev, opt_f);
     if (maximize) {
         opt->maximize = maximize;
-        opt->negate = 0;
+        obj.negate = false;
         opt->stopval = -opt->stopval;
-        opt->f = f0;
-        opt->f_data = d0;
+        obj.f = f0;
+        obj.data = d0;
         *opt_f = -*opt_f;
     }
     return ret;
@@ -1112,8 +1035,8 @@ nlopt_result run_ccsa(nlopt_opt opt, double *x_host, double *x_dev, double *minf
         return NLOPT_INVALID_ARGS;
     }
     if (n == 0) {                                    /* optimize.c:536-539 */
-        if (!opt->f) { set_err(opt, "n == 0 needs a host objective"); return NLOPT_INVALID_ARGS; }
-        *minf = opt->f(0, x_host, nullptr, opt->f_data);
+        if (!opt->objective.f) { set_err(opt, "n == 0 needs a host objective"); return NLOPT_INVALID_ARGS; }
+        *minf = opt->objective.f(0, x_host, nullptr, opt->objective.data);
         return NLOPT_SUCCESS;
     }
     *minf = HUGE_VAL;
@@ -1170,12 +1093,13 @@ nlopt_result run_ccsa(nlopt_opt opt, double *x_host, double *x_dev, double *minf
     prm.dual_xtol_abs = nlopt_get_param(opt, "dual_xtol_abs", 0.0);
     prm.dual_maxeval = (int) nlopt_get_param(opt, "dual_maxeval", lo ? (double) lo->maxeval : 100000.0);
 
-    bool any_pre = opt->pre != nullptr;
-    for (const auto &c : opt->fc) any_pre = any_pre || c.pre != nullptr;
+    bool any_pre = opt->objective.pre != nullptr, all_host = opt->objective.host();
+    for (const auto &c : opt->fc) {
+        any_pre = any_pre || c.fn.pre != nullptr;
+        all_host = all_host && c.fn.host();
+    }
     if (any_pre && opt->algorithm == NLOPT_LD_CCSAQ) {          /* ccsa_quadratic.c: the !no_precond branch */
-        bool dev_c = false;                                     /* device (scalar or vector) or sharded constraints */
-        for (const auto &c : opt->fc) dev_c = dev_c || c.df;
-        if (!x_host || opt->df || dev_c) {
+        if (!x_host || !all_host) {
             set_err(opt, "preconditioned CCSAQ takes host x and host callbacks (nlopt_precond is a host function)");
             return NLOPT_INVALID_ARGS;
         }
@@ -1191,22 +1115,11 @@ nlopt_result run_ccsa(nlopt_opt opt, double *x_host, double *x_dev, double *minf
     nb200::BackendConfig cfg;
     cfg.variant = opt->algorithm == NLOPT_LD_MMA ? nb200::kMMA : nb200::kCCSAQ;
     cfg.n = n;
-    cfg.objective.f = opt->f;
-    cfg.objective.df = opt->df;
-    cfg.objective.df2 = opt->df2;
-    cfg.objective.dfin = opt->dfin;
-    cfg.objective.dtf = opt->dtf;
-    cfg.objective.halo = opt->halo;
-    cfg.objective.sf = opt->sf;
-    cfg.objective.data = opt->f_data;
-    cfg.objective.negate = opt->negate != 0;
+    cfg.objective = opt->objective;
     cfg.penalty = opt->penalty;
     std::vector<double> tol;
     for (const auto &c : opt->fc) {
-        nb200::FuncSpec s;
-        s.m = c.m; s.f = c.f; s.mf = c.mf; s.df = c.df; s.df2 = c.df2; s.dfin = c.dfin; s.dmf2 = c.dmf2; s.dmfin = c.dmfin;
-        s.dtf = c.dtf; s.halo = c.halo; s.sf = c.sf; s.data = c.f_data;
-        cfg.constraints.push_back(s);
+        cfg.constraints.push_back(c.fn);
         tol.insert(tol.end(), c.tol.begin(), c.tol.end());
     }
     cfg.lb = opt->lb.data();
@@ -1334,15 +1247,13 @@ struct PrecondModel {
     const double *x0 = nullptr, *sigma = nullptr, *dfdx = nullptr, *dfcdx = nullptr;
     double fval = 0, rho = 0;
     const double *fcval = nullptr, *rhoc = nullptr;
-    nlopt_precond pre = nullptr;
-    void *pre_data = nullptr;
-    std::vector<nlopt_precond> prec;
-    std::vector<void *> prec_data;
+    const FuncSpec *obj = nullptr;           // the preconditioners (and their data) of the objective ...
+    std::vector<const FuncSpec *> prec;      // ... and of each constraint row
     std::vector<double> scratch;             // dx | H dx
     long count = 0;
 };
 
-double precond_gfunc(PrecondModel &d, double f, const double *dfdx, double rho, nlopt_precond pre, void *pre_data, const double *x,
+double precond_gfunc(PrecondModel &d, double f, const double *dfdx, double rho, const FuncSpec &fn, const double *x,
                      double *grad)                                     // ccsa_quadratic.c:153-181
 {
     const unsigned n = d.n;
@@ -1354,8 +1265,8 @@ double precond_gfunc(PrecondModel &d, double f, const double *dfdx, double rho, 
         val += dfdx[j] * dx[j] + (0.5 * rho) * (dx[j] * dx[j]) * sigma2inv;
         if (grad) grad[j] = dfdx[j] + rho * dx[j] * sigma2inv;
     }
-    if (pre) {
-        pre(n, d.x0, dx, Hdx, pre_data);
+    if (fn.pre) {
+        fn.pre(n, d.x0, dx, Hdx, fn.data);
         for (unsigned j = 0; j < n; ++j) val += 0.5 * dx[j] * Hdx[j];
         if (grad)
             for (unsigned j = 0; j < n; ++j) grad[j] += Hdx[j];
@@ -1367,14 +1278,14 @@ double precond_g0(unsigned, const double *x, double *grad, void *dp)     // :183
 {
     PrecondModel &d = *static_cast<PrecondModel *>(dp);
     ++d.count;
-    return precond_gfunc(d, d.fval, d.dfdx, d.rho, d.pre, d.pre_data, x, grad);
+    return precond_gfunc(d, d.fval, d.dfdx, d.rho, *d.obj, x, grad);
 }
 
 void precond_gi(unsigned m, double *result, unsigned n, const double *x, double *grad, void *dp)      // :194-206
 {
     PrecondModel &d = *static_cast<PrecondModel *>(dp);
     for (unsigned i = 0; i < m; ++i)
-        result[i] = precond_gfunc(d, d.fcval[i], d.dfcdx + (size_t) i * n, d.rhoc[i], d.prec[i], d.prec_data[i], x,
+        result[i] = precond_gfunc(d, d.fcval[i], d.dfcdx + (size_t) i * n, d.rhoc[i], *d.prec[i], x,
                                   grad ? grad + (size_t) i * n : nullptr);
 }
 
@@ -1382,7 +1293,7 @@ nlopt_result run_ccsa_precond(nlopt_opt opt, double *x, double *minf, const nb20
 {
     const unsigned n = opt->n;
     unsigned m = 0;
-    for (const auto &c : opt->fc) m += c.m;
+    for (const auto &c : opt->fc) m += c.fn.m;
     const double t_start = nb200::wall_seconds();
     opt->stats = nlopt_b200_stats{};
     opt->numevals = 0;
@@ -1397,9 +1308,9 @@ nlopt_result run_ccsa_precond(nlopt_opt opt, double *x, double *minf, const nb20
     dd.n = n; dd.m = m;
     dd.x0 = x; dd.sigma = sigma.data(); dd.dfdx = dfdx.data(); dd.dfcdx = dfcdx.data();
     dd.fcval = fcval.data(); dd.rhoc = rhoc.data();
-    dd.pre = opt->pre; dd.pre_data = opt->f_data;
+    dd.obj = &opt->objective;
     for (const auto &c : opt->fc)
-        for (unsigned k = 0; k < c.m; ++k) { dd.prec.push_back(c.pre); dd.prec_data.push_back(c.f_data); }
+        for (unsigned k = 0; k < c.fn.m; ++k) dd.prec.push_back(&c.fn);
     dd.scratch.assign(2 * (size_t) n, 0.0);
 
     // the nested optimiser (ccsa_quadratic.c:299-324): dual algorithm and tolerances, objective g0, constraints gi
@@ -1421,13 +1332,13 @@ nlopt_result run_ccsa_precond(nlopt_opt opt, double *x, double *minf, const nb20
         sigma[j] = sigma[j] > prm.sigma_min ? sigma[j] : prm.sigma_min;
     }
     double rho = prm.rho_init, fcur;
-    auto eval_f = [&](const double *xx, double *g) { ++opt->numevals; return opt->f(n, xx, g, opt->f_data); };
+    const FuncSpec &obj = opt->objective;
+    auto eval_f = [&](const double *xx, double *g) { ++opt->numevals; return obj.f(n, xx, g, obj.data); };
     auto eval_c = [&](const double *xx, double *vals, double *grads) -> bool {
         unsigned i = 0;
         for (const auto &c : opt->fc) {
-            if (c.f) vals[i] = c.f(n, xx, grads ? grads + (size_t) i * n : nullptr, c.f_data);
-            else c.mf(c.m, vals + i, n, xx, grads ? grads + (size_t) i * n : nullptr, c.f_data);
-            i += c.m;
+            eval_host(c.fn, n, xx, vals + i, grads ? grads + (size_t) i * n : nullptr);
+            i += c.fn.m;
             if (forced()) return false;
         }
         return true;
@@ -1502,7 +1413,7 @@ nlopt_result run_ccsa_precond(nlopt_opt opt, double *x, double *minf, const nb20
                 : inner_done;
             if (take) {                               // :500-545
                 if (!prm.inner_gradients) {
-                    fcur = opt->f(n, xcur.data(), dfdx_cur.data(), opt->f_data);
+                    fcur = obj.f(n, xcur.data(), dfdx_cur.data(), obj.data);
                     if (forced()) return NLOPT_FORCED_STOP;
                     if (!eval_c(xcur.data(), fcval_cur.data(), dfcdx_cur.data())) return NLOPT_FORCED_STOP;
                 }
@@ -1576,13 +1487,6 @@ bool stop_x_host(const nlopt_opt opt, const double *x, const double *oldx)      
     return true;
 }
 
-// nlopt_eval_constraint without gradient (stop.c:178-184)
-void eval_values(const nb200::ConstraintRec &c, unsigned n, const double *x, double *out)
-{
-    if (c.f) out[0] = c.f(n, x, nullptr, c.f_data);
-    else c.mf(c.m, out, n, x, nullptr, c.f_data);
-}
-
 // x_dev: the sub-problem starts from (and returns into) this device array instead of host x
 nlopt_result optimize_limited(nlopt_opt sub, double *x, double *x_dev, double *minf, int maxeval, double maxtime)   // optimize.c:1087-1113
 {
@@ -1606,11 +1510,11 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
     const unsigned n = opt->n;
     const nlopt_algorithm alg = opt->algorithm;
     if (opt->maximize || (!x && !x_dev)) { set_err(opt, "NULL args to nlopt_optimize_"); return NLOPT_INVALID_ARGS; }
-    bool dev = x_dev != nullptr || opt->df != nullptr, sharded = opt->sf != nullptr;
+    bool dev = x_dev != nullptr || !opt->objective.host(), sharded = opt->objective.sharded();
     for (const auto *list : {&opt->fc, &opt->h})
         for (const auto &c : *list) {
-            dev = dev || c.df;
-            sharded = sharded || c.sf;
+            dev = dev || !c.fn.host();
+            sharded = sharded || c.fn.sharded();
         }
     if (sharded) {
         set_err(opt, "NLOPT_AUGLAG* does not take sharded host callbacks (nlopt_b200_sfunc) in this library");
@@ -1660,7 +1564,7 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
         ~Cleanup()
         {
             sub->penalty = nullptr;
-            sub->negate = 0;
+            sub->objective.negate = false;
             opt->force_stop_child = nullptr;
             if (own) nlopt_destroy(sub);
         }
@@ -1685,19 +1589,13 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
     const std::vector<nb200::ConstraintRec> &pen_fc = sub_has_fc ? none : opt->fc;     /* auglag.c:98-101 */
     const std::vector<nb200::ConstraintRec> &sub_fc = sub_has_fc ? opt->fc : none;
     unsigned mm = 0, pp = 0;
-    for (const auto &c : pen_fc) mm += c.m;
-    for (const auto &c : opt->h) pp += c.m;
+    for (const auto &c : pen_fc) mm += c.fn.m;
+    for (const auto &c : opt->h) pp += c.fn.m;
 
     nb200::PenaltySpec pen;
     std::vector<double> lambda(pp ? pp : 1, 0.0), mu(mm ? mm : 1, 0.0);
-    auto to_spec = [](const nb200::ConstraintRec &c) {
-        nb200::FuncSpec s;
-        s.m = c.m; s.f = c.f; s.mf = c.mf; s.df = c.df; s.df2 = c.df2; s.dfin = c.dfin; s.dmf2 = c.dmf2; s.dmfin = c.dmfin;
-        s.dtf = c.dtf; s.halo = c.halo; s.data = c.f_data;
-        return s;
-    };
-    for (const auto &c : opt->h) pen.eq.push_back(to_spec(c));
-    for (const auto &c : pen_fc) pen.ineq.push_back(to_spec(c));
+    for (const auto &c : opt->h) pen.eq.push_back(c.fn);
+    for (const auto &c : pen_fc) pen.ineq.push_back(c.fn);
     pen.lambda = lambda.data();
     pen.mu = mu.data();
     opt->numevals = 0;
@@ -1706,16 +1604,9 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
 
     /* configure the sub-optimiser (auglag.c:107-137).  Its objective is f + penalties: f goes in as its plain
        objective, the rest as the penalty spec */
-    sub->f = opt->f;
-    sub->f_data = opt->f_data;
-    sub->df = opt->df;
-    sub->df2 = opt->df2;
-    sub->dfin = opt->dfin;
-    sub->dtf = opt->dtf;
-    sub->halo = opt->halo;
-    sub->pre = nullptr;
+    sub->objective = opt->objective;    /* negate too: a maximised device objective's sub-problem L starts from -f */
+    sub->objective.pre = nullptr;       /* auglag.c:109-135: the sub-problem takes no preconditioner */
     sub->maximize = 0;
-    sub->negate = opt->negate;          /* a maximised device objective: the sub-problem's L starts from -f */
     if (dev_bounds) {                                /* D2D into the sub-optimiser, which is then in device mode */
         std::string err;
         if (!opt->dbounds->copy_into(&sub->dbounds, &err)) {
@@ -1741,13 +1632,9 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
         sub->munge_on_copy = mc;
     }
     for (const auto &c : sub_fc) {
-        nlopt_result r = c.dmf2 ? nlopt_b200_add_inequality_mconstraint_device2(sub, c.m, c.dmf2, c.dmfin, c.f_data, c.tol.data(), c.halo)
-                       : c.dtf && c.dmfin ? nlopt_b200_add_inequality_mconstraint_terms(sub, c.m, c.dtf, c.dmfin, c.f_data, c.tol.data(), c.halo)
-                       : c.dtf ? nlopt_b200_add_inequality_constraint_terms(sub, c.dtf, c.dfin, c.f_data, c.tol[0], c.halo)
-                       : c.df2 ?nlopt_b200_add_inequality_constraint_device2(sub, c.df2, c.dfin, c.f_data, c.tol[0], c.halo)
-                       : c.df  ? nlopt_b200_add_inequality_constraint_device(sub, c.df, c.f_data, c.tol[0])
-                       : c.f   ? nlopt_add_inequality_constraint(sub, c.f, c.f_data, c.tol[0])
-                               : nlopt_add_inequality_mconstraint(sub, c.m, c.mf, c.f_data, c.tol.data());
+        FuncSpec fn = c.fn;
+        fn.pre = nullptr;                   /* as the objective's */
+        const nlopt_result r = add_any(sub, false, fn, c.tol.data());
         if (r < 0) return r;
     }
     sub->penalty = &pen;
@@ -1759,10 +1646,9 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
         nb200::BackendConfig vc;
         vc.values_only = true;
         vc.n = n;
-        vc.objective.f = opt->f; vc.objective.df = opt->df; vc.objective.df2 = opt->df2; vc.objective.dfin = opt->dfin;
-        vc.objective.dtf = opt->dtf; vc.objective.halo = opt->halo; vc.objective.data = opt->f_data; vc.objective.negate = opt->negate != 0;
-        for (const auto &c : opt->h) vc.constraints.push_back(to_spec(c));
-        for (const auto &c : pen_fc) vc.constraints.push_back(to_spec(c));
+        vc.objective = opt->objective;
+        for (const auto &c : opt->h) vc.constraints.push_back(c.fn);
+        for (const auto &c : pen_fc) vc.constraints.push_back(c.fn);
         vc.lb = opt->lb.data();
         vc.ub = opt->ub.data();
         vc.x0_host = x;
@@ -1791,18 +1677,18 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
     auto eval_point = [&](double *f) -> nlopt_result {
         ++opt->numevals;
         if (!dev) {
-            *f = opt->f(n, xcur.data(), nullptr, opt->f_data);
+            *f = opt->objective.f(n, xcur.data(), nullptr, opt->objective.data);
             if (forced()) return NLOPT_FORCED_STOP;
             unsigned i = 0;
             for (const auto &c : opt->h) {
-                eval_values(c, n, xcur.data(), hv.data() + i);
-                i += c.m;
+                eval_host(c.fn, n, xcur.data(), hv.data() + i, nullptr);
+                i += c.fn.m;
                 if (forced()) return NLOPT_FORCED_STOP;
             }
             i = 0;
             for (const auto &c : pen_fc) {
-                eval_values(c, n, xcur.data(), cv.data() + i);
-                i += c.m;
+                eval_host(c.fn, n, xcur.data(), cv.data() + i, nullptr);
+                i += c.fn.m;
                 if (forced()) return NLOPT_FORCED_STOP;
             }
             return NLOPT_SUCCESS;
@@ -1855,7 +1741,7 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
             feasible = 1;
             unsigned ii = 0;
             for (const auto &c : opt->h)
-                for (unsigned k = 0; k < c.m; ++k) {
+                for (unsigned k = 0; k < c.fn.m; ++k) {
                     const double hi = hv[ii++];
                     penalty += std::fabs(hi);
                     feasible = feasible && std::fabs(hi) <= c.tol[k];
@@ -1863,7 +1749,7 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
                 }
             ii = 0;
             for (const auto &c : pen_fc)
-                for (unsigned k = 0; k < c.m; ++k) {
+                for (unsigned k = 0; k < c.fn.m; ++k) {
                     const double fci = cv[ii++];
                     penalty += fci > 0 ? fci : 0;
                     feasible = feasible && fci <= c.tol[k];
@@ -1892,7 +1778,7 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
             feasible = 1;
             unsigned ii = 0;
             for (const auto &c : opt->h)
-                for (unsigned k = 0; k < c.m; ++k) {
+                for (unsigned k = 0; k < c.fn.m; ++k) {
                     const double hi = hv[ii];
                     const double newlam = lambda[ii] + pen.rho * hi;
                     penalty += std::fabs(hi);
@@ -1902,7 +1788,7 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
                 }
             ii = 0;
             for (const auto &c : pen_fc)
-                for (unsigned k = 0; k < c.m; ++k) {
+                for (unsigned k = 0; k < c.fn.m; ++k) {
                     const double fci = cv[ii];
                     const double newmu = mu[ii] + pen.rho * fci;
                     penalty += fci > 0 ? fci : 0;

@@ -13,20 +13,8 @@ namespace nb200 {
 
 // one registered constraint object (reference: nlopt_constraint, src/util/nlopt-util.h:119-126)
 struct ConstraintRec {
-    unsigned m = 1;                 // output dimension
-    nlopt_func f = nullptr;         // scalar host callback
-    nlopt_mfunc mf = nullptr;       // vector host callback
-    nlopt_b200_dfunc df = nullptr;  // scalar device callback (extension)
-    nlopt_b200_dfunc2 df2 = nullptr;    // asynchronous form (df then holds a marker)
-    nlopt_b200_dfinish dfin = nullptr;
-    nlopt_b200_dmfunc2 dmf2 = nullptr;  // vector asynchronous form, m rows (df then holds a marker)
-    nlopt_b200_dmfinish dmfin = nullptr;
-    nlopt_b200_dtfunc dtf = nullptr;    // per-variable terms, m rows (df holds a marker; finish in dfin, or dmfin for the vector form)
-    int halo = 0;
-    nlopt_b200_sfunc sf = nullptr;      // sharded host callback (df then holds a marker)
-    nlopt_precond pre = nullptr;
-    void *f_data = nullptr;
-    std::vector<double> tol;        // m feasibility tolerances
+    FuncSpec fn;
+    std::vector<double> tol;        // fn.m feasibility tolerances
 };
 
 struct NamedParam {
@@ -48,17 +36,8 @@ struct nlopt_opt_s {
     nlopt_algorithm algorithm;
     unsigned n;
 
-    nlopt_func f = nullptr;
-    nlopt_b200_dfunc df = nullptr;
-    nlopt_b200_dfunc2 df2 = nullptr;
-    nlopt_b200_dfinish dfin = nullptr;
-    nlopt_b200_dtfunc dtf = nullptr;        // per-variable terms (finish in dfin)
-    int halo = 0;
-    nlopt_b200_sfunc sf = nullptr;
-    void *f_data = nullptr;
-    nlopt_precond pre = nullptr;
+    nb200::FuncSpec objective;      // negate: while a maximisation with a device or sharded objective runs
     int maximize = 0;
-    int negate = 0;         // while a maximisation with a device or sharded objective runs: the backend negates f
 
     std::vector<nb200::NamedParam *> params;      // pointers stay valid: nlopt_nth_param hands out c_str()
 
