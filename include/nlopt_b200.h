@@ -482,7 +482,8 @@ int nlopt_b200_dual_end_outer(nlopt_b200_dual h, int k, double sigma_min, const 
 int nlopt_b200_dual_set_prev(nlopt_b200_dual h, const double *xcur, const double *xprev, const double *xprevprev);
 /* timing helper: average device milliseconds of `iters` back-to-back evaluations (CUDA events) */
 int nlopt_b200_dual_time(nlopt_b200_dual h, const double *y, int want_xcur, int iters, double *ms_avg);
-/* tuning knobs for the launch geometry (0 = default); returns 0 on success */
+/* tuning knobs for the launch geometry (0 = default); returns 0 on success.  "scalar_bounds" 1: the uploaded bounds
+ * are uniform (checked) and reach the dual kernels as two scalars, as bounds set with nlopt_set_*_bounds1 do */
 int nlopt_b200_dual_configure(nlopt_b200_dual h, const char *key, long long value);
 long long nlopt_b200_dual_query(nlopt_b200_dual h, const char *key);
 

@@ -42,7 +42,8 @@ constexpr int kWarps = kBlock / 32;
 constexpr int kVirtualShards = 8;        // V: fixed, so 1/2/4/8 ranks give bit-identical sums
 constexpr int kMaxParamM = 16;           // multipliers that travel as kernel parameters (register-row kernels); m > 16: wide kernel
 constexpr int kMaxNV = 3 + kMaxParamM;   // accumulators one CTA of the register-row kernels carries: val, g0, w, <=16 g_i
-constexpr int kWideMaxM = 2048;          // the wide kernel keeps its per-row scalars in shared memory (88 bytes per row)
+constexpr int kWideMaxM = 2048;          // the wide kernel keeps 96 bytes of shared memory per row: 4 per-row scalars and the
+                                         // 8 warps' row sums; 192 KiB of dynamic shared memory at m = 2048
 
 // ---- exact-rounding arithmetic (never fused) ---------------------------------------------
 __device__ __forceinline__ double mulx(double a, double b) { return __dmul_rn(a, b); }

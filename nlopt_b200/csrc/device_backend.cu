@@ -301,7 +301,8 @@ bool DeviceBackend::alloc_state()
         if (gr.ld > shard_cap_) shard_cap_ = gr.ld;
     }
     if (m_ > (unsigned) kWideMaxM)
-        return fail("more than 2048 inequality constraints: the dual kernel keeps 88 bytes of shared memory per constraint");
+        return fail("more than 2048 inequality constraints: the dual kernel keeps 96 bytes of shared memory per constraint "
+                    "(192 KiB at m = 2048)");
 
     NB_CUDA(cudaDeviceGetAttribute(&sm_count_, cudaDevAttrMultiProcessorCount, device_));
     NB_CUDA(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
@@ -1711,8 +1712,31 @@ bool DeviceBackend::upload(const char *which, const double *host)
     if (std::string(which) == "xcur") { dst = xcur_; cand_in_x_ = false; }
     if (!dst) return fail(std::string("unknown array ") + which);
     if (dst == sigma_) sidx_valid_ = false;
+    if (dst == lb_ || dst == ub_) set_scalar_bounds(false);     // new bounds: arrays until scalar_bounds is set again
     NB_CUDA(cudaMemcpyAsync(dst, host + geo_.j0, geo_.n_local * sizeof(double), cudaMemcpyHostToDevice, stream_));
     NB_CUDA(cudaStreamSynchronize(stream_));
+    return true;
+}
+
+// The kernel-level handle uploads bounds as arrays.  scalar_bounds = 1 reads them back and, when every lb and every ub
+// entry of the shard has the bits of its first one, hands them to the dual kernels as two scalars -- the instantiations
+// nlopt_optimize picks for bounds set with nlopt_set_*_bounds1.  0 goes back to the arrays.
+bool DeviceBackend::set_scalar_bounds(bool on)
+{
+    scalar_bounds_ = false;
+    lb_u_ = ub_u_ = 0.0;
+    if (!on) return true;
+    std::vector<double> lb(geo_.n_local), ub(geo_.n_local);
+    NB_CUDA(cudaMemcpyAsync(lb.data(), lb_, geo_.n_local * sizeof(double), cudaMemcpyDeviceToHost, stream_));
+    NB_CUDA(cudaMemcpyAsync(ub.data(), ub_, geo_.n_local * sizeof(double), cudaMemcpyDeviceToHost, stream_));
+    NB_CUDA(cudaStreamSynchronize(stream_));
+    for (size_t j = 1; j < lb.size(); ++j)
+        if (std::memcmp(&lb[j], &lb[0], sizeof(double)) || std::memcmp(&ub[j], &ub[0], sizeof(double)))
+            return fail("scalar_bounds: the bounds are not uniform");
+    if (lb.empty()) return fail("scalar_bounds: empty shard");
+    scalar_bounds_ = true;
+    lb_u_ = lb[0];
+    ub_u_ = ub[0];
     return true;
 }
 
@@ -1764,6 +1788,7 @@ bool DeviceBackend::configure(const char *key, long long value)
     if (k == "solve_tma") { solve_tma_ = (int) value; return true; }
     if (k == "solve_async") { solve_async_ = (int) value; return true; }
     if (k == "solve_minb") { solve_minb_ = (int) value; return true; }
+    if (k == "scalar_bounds") return set_scalar_bounds(value != 0);
     if (k == "l2_keep_mb") {
         l2_keep_bytes_ = value <= 0 ? 0 : (size_t) value << 20;
         // evict_last lines are only protected inside the persisting carve-out of the L2: size it to the request

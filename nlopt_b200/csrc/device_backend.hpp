@@ -73,6 +73,7 @@ public:
                          const double *xtol_abs_dev = nullptr);
     bool time_dual(const double *y, const DualScalars &sc, bool materialize, int iters, double *ms_avg);
     bool configure(const char *key, long long value) override;
+    bool set_scalar_bounds(bool on);
     long long query(const char *key) const;
     const Geometry &geometry() const { return geo_; }
     bool is_mma() const { return variant_ == kMMA; }
