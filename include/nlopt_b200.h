@@ -318,7 +318,8 @@ nlopt_result nlopt_b200_add_equality_mconstraint_device2(nlopt_opt opt, unsigned
  * bit for bit (result code, evaluation counts, f*, x*) under LD_MMA, LD_CCSAQ and the AUGLAG family; the value depends
  * on n only, not on the number of ranks.  `halo` as for the _device2 forms (the callback may read x_dev[-1] and
  * x_dev[n_local]).  Argument checks are those of the _device2 / _mconstraint_device2 twins; any m the constraint path
- * accepts (no register-file cap).  Not taken by preconditioned CCSAQ. */
+ * accepts (no register-file cap).  Not taken by preconditioned CCSAQ with host preconditioners only (nlopt_precond; the
+ * device preconditioners below take every callback form). */
 typedef void (*nlopt_b200_dtfunc)(unsigned m, const nlopt_b200_shard *shard, const double *x_dev, double *grad_dev,
                                   unsigned long long ld, double *terms_dev, void *func_data, void *cuda_stream);
 nlopt_result nlopt_b200_set_min_objective_terms(nlopt_opt opt, nlopt_b200_dtfunc f, nlopt_b200_dfinish finish,
@@ -335,6 +336,28 @@ nlopt_result nlopt_b200_add_inequality_mconstraint_terms(nlopt_opt opt, unsigned
 nlopt_result nlopt_b200_add_equality_mconstraint_terms(nlopt_opt opt, unsigned m, nlopt_b200_dtfunc h,
                                                        nlopt_b200_dmfinish finish, void *h_data, const double *tol,
                                                        int halo);
+/* Device preconditioners for NLOPT_LD_CCSAQ (the device twin of nlopt_precond, reference nlopt.h:70): with one on the
+ * objective or on an inequality constraint, CCSAQ's convex model of that function around the accepted point x0 gains the
+ * term 1/2 dx^T H(x0) dx (ccsa_quadratic.c:153-206), and each inner iteration solves the model problem with a nested
+ * LD_MMA run whose variables, bounds, model values and gradients stay in GPU memory.  The callback computes
+ * vpre = H(x) v on the device: it enqueues on cuda_stream and does not synchronise.  x_dev is the model centre (the
+ * accepted point), v_dev = dx, vpre_dev a library buffer of n_local doubles, valid for the call and the work it
+ * enqueues.  The library calls it once per preconditioned function per model evaluation.
+ * The preconditioner is attached to the function's record: it works with every objective form (host, device, _device2,
+ * terms, JIT, torch) and every inequality form of one row, and a later registration that replaces the record drops it.
+ * For a maximised objective the callback computes H of the function to maximise and the library applies -H (one
+ * negation of vpre on the stream), so maximising (-F, -H) runs bit for bit like minimising (F, H).  pre == NULL clears
+ * the record's device preconditioner.  pre_data stays the caller's: the munge hooks (nlopt_set_munge) never see it, and
+ * nlopt_copy shares it with the copy, so it must outlive both objects.  NLOPT_INVALID_ARGS, with a message: no objective registered, an index out of
+ * range, a vector (m > 1) record, a record with a host preconditioner (nlopt_precond; a record takes one of the two).
+ * Equality constraints take none (the AUGLAG sub-problem drops preconditioners, auglag.c:109-135), LD_MMA ignores them
+ * (mma.c), and a run with both host and device preconditioners, or on several ranks, is NLOPT_INVALID_ARGS. */
+typedef void (*nlopt_b200_dprecond)(const nlopt_b200_shard *shard, const double *x_dev, const double *v_dev,
+                                    double *vpre_dev, void *pre_data, void *cuda_stream);
+nlopt_result nlopt_b200_set_objective_precond_device(nlopt_opt opt, nlopt_b200_dprecond pre, void *pre_data);
+/* index: the index-th inequality-constraint record, in registration order */
+nlopt_result nlopt_b200_set_constraint_precond_device(nlopt_opt opt, unsigned index, nlopt_b200_dprecond pre,
+                                                      void *pre_data);
 /* Device functors given as SOURCE, for callers without nvcc.  nlopt_b200_jit_create compiles `source` with NVRTC
  * (opened at the first call; libnvrtc.so.12 by soname, else from the toolkit the library was built with) for sm_90a,
  * with -std=c++17 --fmad=false and the caller's options, together with the map kernels of
@@ -397,7 +420,7 @@ nlopt_result nlopt_b200_optimize_device(nlopt_opt opt, double *x_dev, double *op
  * lane 0.  Any host bound setter downloads both arrays and leaves device mode; nlopt_get_*_bounds,
  * nlopt_set_local_optimizer and the initial-step heuristics read the device values; nlopt_copy duplicates them.
  * NULL: NLOPT_INVALID_ARGS; n == 0: no-op; no usable device: NLOPT_FAILURE, bounds unchanged; several ranks, a run on
- * another current device, or preconditioned CCSAQ: NLOPT_INVALID_ARGS.  The deprecated nlopt_minimize* API takes host
+ * another current device, or preconditioned CCSAQ with host preconditioners only (nlopt_precond): NLOPT_INVALID_ARGS.  The deprecated nlopt_minimize* API takes host
  * bounds only. */
 nlopt_result nlopt_b200_set_lower_bounds_device(nlopt_opt opt, const double *lb_dev);
 nlopt_result nlopt_b200_set_upper_bounds_device(nlopt_opt opt, const double *ub_dev);

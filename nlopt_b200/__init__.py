@@ -17,8 +17,8 @@ import ctypes as C
 
 import numpy as np
 
-from ._capi import (NLOPT_B200_DFINISH, NLOPT_B200_DFUNC, NLOPT_B200_DMFINISH, NLOPT_B200_DTFUNC, NLOPT_FUNC,
-                    NLOPT_PRECOND, NLOPT_MFUNC, Library, Shard, Stats, c_double_p, default_library)
+from ._capi import (NLOPT_B200_DFINISH, NLOPT_B200_DFUNC, NLOPT_B200_DMFINISH, NLOPT_B200_DPRECOND, NLOPT_B200_DTFUNC,
+                    NLOPT_FUNC, NLOPT_PRECOND, NLOPT_MFUNC, Library, Shard, Stats, c_double_p, default_library)
 
 # --- algorithm ids (reference nlopt.h:72-154) ---------------------------------
 _ALG_NAMES = [
@@ -53,6 +53,13 @@ def _as_f64(a, n=None):
     if n is not None and a.size != n:
         raise ValueError(f"dimension mismatch: expected {n}, got {a.size}")
     return a
+
+
+def _index(i):
+    """a constraint record index for the C ABI (unsigned)"""
+    if isinstance(i, bool) or not isinstance(i, (int, np.integer)) or not 0 <= int(i) < 2 ** 32:
+        raise ValueError(f"a constraint index is an integer in [0, 2**32), got {i!r}")
+    return int(i)
 
 
 def _ptr(a):
@@ -374,6 +381,45 @@ class opt:
         tol = _as_f64(tol)
         self._check(self._lib.nlopt_b200_add_equality_mconstraint_terms(
             self._h, tol.size, self._wrap_terms(h, True, halo), self._wrap_mfinish(finish), None, _ptr(tol), int(halo)))
+
+    # ---- extension: device preconditioners of LD_CCSAQ (nlopt_b200_dprecond) -----------------------------------------
+    # pre(x, v, vpre) gets float64 CUDA views of the library's buffers -- x the model centre, v = dx, vpre (n_local
+    # entries each) -- and writes vpre = H(x) v in place, on the library's stream (torch.cuda.ExternalStream).  The
+    # pointer forms take an nlopt_b200_dprecond address and its data; None clears the record's preconditioner.
+    def _wrap_dprecond(self, pre):
+        import torch
+
+        def view(ptr, n):
+            return self._tcached((ptr, (n,), (8,)), lambda: torch.as_tensor(_DeviceArray(ptr, (n,), (8,))))
+
+        def thunk(shard, x, v, vpre, _data, stream):
+            try:
+                n = Shard.from_address(shard).n_local
+                xv, vv, pv = view(x, n), view(v, n), view(vpre, n)
+                with torch.cuda.stream(self._tcached(("stream", stream), lambda: torch.cuda.ExternalStream(stream, device=xv.device))):
+                    pre(xv, vv, pv)
+            except BaseException as e:
+                self._exc = e
+                self._lib.nlopt_force_stop(self._h)
+
+        cb = NLOPT_B200_DPRECOND(thunk)
+        self._keep.append(cb)
+        return C.cast(cb, C.c_void_p)
+
+    def set_objective_precond_device(self, fn_ptr, data_ptr=None):
+        self._check(self._lib.nlopt_b200_set_objective_precond_device(self._h, fn_ptr, data_ptr))
+
+    def set_constraint_precond_device(self, index, fn_ptr, data_ptr=None):
+        self._check(self._lib.nlopt_b200_set_constraint_precond_device(self._h, _index(index), fn_ptr, data_ptr))
+
+    def set_objective_precond_torch(self, pre):
+        fn = None if pre is None else self._wrap_dprecond(pre)
+        self._check(self._lib.nlopt_b200_set_objective_precond_device(self._h, fn, None))
+
+    def set_constraint_precond_torch(self, index, pre):
+        index = _index(index)
+        fn = None if pre is None else self._wrap_dprecond(pre)
+        self._check(self._lib.nlopt_b200_set_constraint_precond_device(self._h, index, fn, None))
 
     # ---- extension: __device__ functors given as source (CudaFunctor, nlopt_b200_jit) ---------------------------------
     # params: the functor object's bytes (sizeof(F) of them; e.g. bytes(ctypes.Structure) or struct.pack, with

@@ -24,6 +24,8 @@ NLOPT_B200_DTFUNC = C.CFUNCTYPE(None, C.c_uint, C.c_void_p, C.c_void_p, C.c_void
                                 C.c_void_p, C.c_void_p)
 NLOPT_B200_DFINISH = C.CFUNCTYPE(C.c_double, C.c_double, C.c_void_p)
 NLOPT_B200_DMFINISH = C.CFUNCTYPE(None, C.c_uint, c_double_p, c_double_p, C.c_void_p)
+# device preconditioners (nlopt_b200_dprecond): shard, x0, v, vpre, data, stream
+NLOPT_B200_DPRECOND = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p)
 
 
 class Shard(C.Structure):
@@ -175,6 +177,8 @@ _EXT = {
         (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p, c_double_p, C.c_int]),
     "nlopt_b200_add_equality_mconstraint_terms":
         (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p, c_double_p, C.c_int]),
+    "nlopt_b200_set_objective_precond_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "nlopt_b200_set_constraint_precond_device": (C.c_int, [C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p]),
     # __device__ functors given as source, compiled at run time (nlopt_b200_jit)
     "nlopt_b200_jit_create": (C.c_void_p, [C.c_char_p, C.c_char_p, C.POINTER(C.c_char_p), C.c_int]),
     "nlopt_b200_jit_destroy": (None, [C.c_void_p]),

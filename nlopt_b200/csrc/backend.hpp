@@ -81,6 +81,26 @@ public:
         return false;
     }
 
+    // Optional, preconditioned CCSAQ (ccsa_quadratic.c:153-206, :299-324, :441-467): a backend whose functions carry
+    // device preconditioners replaces the dual solve of each inner iteration by a model solve.  It minimises the model
+    // g0 subject to gi <= 0 in the trust box max(lb, x - sigma) <= xcur <= min(ub, x + sigma) with a nested LD_MMA run
+    // from xcur = x (tolerances in `stop`), leaves the solution in xcur, and returns g0(xcur) in *gval, gi(xcur) in
+    // gc[m], w = sum 1/2 ((xcur - x) / sigma)^2 in *wval, the nested run's result in *ret and its dual evaluations in
+    // *nevals.  false: the backend failed (message in error()).
+    struct ModelStop {
+        double ftol_rel = 0, ftol_abs = 0;
+        int maxeval = 0;
+        double maxtime = 0;                  // <= 0: unlimited
+        const int *force_stop = nullptr;
+    };
+    virtual bool solves_model() const { return false; }
+    virtual bool model_solve(const DualScalars &sc, const ModelStop &stop, double *gval, double *gc, double *wval, int *ret,
+                             long long *nevals)
+    {
+        (void) sc; (void) stop; (void) gval; (void) gc; (void) wval; (void) ret; (void) nevals;
+        return false;
+    }
+
     // x <- xcur, gradients <- candidate gradients (mma.c:374-377); O(1) buffer swaps
     virtual void accept_candidate() = 0;
 

@@ -29,6 +29,8 @@ struct FuncSpec {
     int halo = 0;
     nlopt_b200_sfunc sf = nullptr;           // sharded host callback
     nlopt_precond pre = nullptr;             // preconditioner of a host function (CCSAQ; the AUGLAG sub-problem has none)
+    nlopt_b200_dprecond dpre = nullptr;      // ... or a device preconditioner, of any form of one row (never both)
+    void *pre_data = nullptr;                // dpre's data
     void *data = nullptr;
     bool negate = false;                     // objective of a maximisation (device / sharded callbacks only): the
                                              // backend minimises -f -- final value and gradient change sign
@@ -85,6 +87,8 @@ struct BackendConfig {
     const double *x_weights_dev = nullptr, *xtol_abs_dev = nullptr;
     nlopt_b200_stats *stats = nullptr;       // h2d/d2h bytes, launches, kernel time
     bool values_only = false;                // x, the best point and the callback workspace only (Backend::point_device)
+    bool maximize = false;                   // the run maximises (any objective form): a device preconditioner's H of the
+                                             // objective changes sign, as its value and gradient do
 };
 
 Backend *make_backend(const BackendConfig &cfg, std::string *err);

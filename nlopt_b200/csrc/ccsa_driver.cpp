@@ -144,6 +144,7 @@ int ccsa_minimize(Variant variant, Backend &be, const std::vector<double> &tol, 
         return assemble(yy, grad);
     };
     bool fused = prm.fused_solve && m > 0 && be.supports_dual_solve();
+    const bool model = variant == kCCSAQ && be.solves_model();     // preconditioned CCSAQ: a model solve per inner iteration
 
     if (!be.first_outer()) return L.fail("state rotation");
     unsigned k = 0;
@@ -159,7 +160,26 @@ int ccsa_minimize(Variant variant, Backend &be, const std::vector<double> &tol, 
             launches = 0;
             bool ok = true;
             const double t_dual0 = wall_seconds();
-            if (fused) {
+            if (model) {
+                // the nested solve of the preconditioned model (ccsa_quadratic.c:441-467); its result as on :455-463
+                Backend::ModelStop ms;
+                ms.ftol_rel = prm.dual_ftol_rel;
+                ms.ftol_abs = prm.dual_ftol_abs;
+                ms.maxeval = prm.dual_maxeval;
+                if (stop.maxtime > 0) {
+                    const double left = stop.maxtime - (wall_seconds() - L.start);
+                    ms.maxtime = left > 0 ? left : 1e-9;
+                }
+                ms.force_stop = stop.force_stop;
+                sc.fval = fbase;
+                sc.rho = rho;
+                int reti = 0;
+                if (!be.model_solve(sc, ms, &g0, gc.data(), &w, &reti, &launches)) return L.fail("model solve");
+                if (reti < 0 || reti == R_MAXTIME) {
+                    if (reti < 0 && errmsg) *errmsg = "nested model solve: " + be.error();
+                    return L.forced() ? R_FORCED : reti;
+                }
+            } else if (fused) {
                 // the whole dual solve + final evaluation as one persistent kernel (SURVEY.md 8(f)-1)
                 const double stop6[6] = {prm.dual_ftol_rel, prm.dual_ftol_abs, prm.dual_xtol_rel, prm.dual_xtol_abs,
                                          (double) prm.dual_maxeval, stop.maxtime - (wall_seconds() - L.start)};
@@ -198,7 +218,7 @@ int ccsa_minimize(Variant variant, Backend &be, const std::vector<double> &tol, 
                     return reti;
                 }
             }
-            if (!fused) {
+            if (!fused && !model) {
                 dual_value(y.data(), nullptr, true, &ok);         // mma.c:288: x*(y), g, w at the solution
                 if (!ok) return L.fail("dual evaluation");
             }
@@ -210,7 +230,7 @@ int ccsa_minimize(Variant variant, Backend &be, const std::vector<double> &tol, 
             const double t_eval0 = wall_seconds();
             if (prm.verbosity) {
                 std::printf("%s dual converged in %lld iterations to g=%g:\n", tag, launches, g0);
-                for (unsigned i = 0; i < m && i < (unsigned) prm.verbosity; ++i)
+                for (unsigned i = 0; i < m && i < (unsigned) prm.verbosity && !model; ++i)
                     std::printf("    %s y[%u]=%g, gc[%u]=%g\n", tag, i, y[i], i, gc[i]);
             }
 

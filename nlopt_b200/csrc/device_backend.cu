@@ -18,7 +18,9 @@
 #include "ccsa_kernels.cuh"
 #include "comm.hpp"
 #include "dual_mma.hpp"
+#include "ccsa_driver.hpp"
 #include "nlopt_object.hpp"
+#include "precond.hpp"
 #include "synth.cuh"
 #include "terms_kernels.cuh"
 
@@ -541,6 +543,20 @@ bool DeviceBackend::setup(const BackendConfig &cfg)
         NB_CUDA(cudaMemsetAsync(sidx_, 0, geo_.ld * sizeof(unsigned short), stream_));
     }
     cand_in_x_ = true;                       // xcur == x at the start (mma.c:220)
+    // device preconditioners under CCSAQ: each inner iteration solves the model problem (model_solve)
+    model_ = PrecondModel();
+    model_.rows.push_back(&cfg_.objective);
+    for (const FuncSpec &c : cfg_.constraints)
+        for (unsigned k = 0; k < c.m; ++k) model_.rows.push_back(&c);
+    for (const FuncSpec *fs : model_.rows) {
+        model_.hrow.push_back(fs->dpre ? (int) model_.npre : -1);
+        if (fs->dpre) ++model_.npre;
+    }
+    model_.on = variant_ == kCCSAQ && !cfg.penalty && model_.npre > 0;
+    model_.negate_h0 = cfg_.maximize;
+    model_.sms = sm_count_;
+    model_fn_[0] = {&model_, 0};
+    model_fn_[1] = {&model_, 1};
     return true;
 }
 
@@ -1571,6 +1587,268 @@ bool DeviceBackend::time_dual(const double *y, const DualScalars &sc, bool mater
     cudaEventDestroy(e1);
     if (materialize) cand_in_x_ = false;
     *ms_avg = (double) ms / iters;
+    return true;
+}
+
+// ------------------------------------------------------------------------------------------------
+// preconditioned CCSAQ (ccsa_quadratic.c:153-206, :299-324, :441-467) with device preconditioners
+//
+// The model problem of one inner iteration is an LD_MMA run of its own DeviceBackend, whose objective g0 and vector
+// constraint gi (m rows) are terms callbacks of this file: per point one dx pass, one preconditioner call per
+// preconditioned row, then one pass per row writing its separable terms into the library's terms buffer (reduced by
+// the nested backend), its gradient, and its quadratic terms, which are reduced here in the same order into the
+// model's own virtual-shard sums.  The finishes add them up as the host path groups its two loops: (f + S) + Q.
+
+
+namespace {
+
+// the 8 virtual-shard sums of a row in index order, as DeviceBackend::finish_evals adds them
+double shard_total(const double *vs)
+{
+    double t = vs[0];
+    for (unsigned v = 1; v < kV; ++v) t += vs[v];
+    return t;
+}
+
+void model_terms(unsigned m, const nlopt_b200_shard *sh, const double *x, double *grad, unsigned long long ld, double *terms,
+                 void *data, void *stream)
+{
+    const DeviceBackend::ModelFn &fn = *static_cast<const DeviceBackend::ModelFn *>(data);
+    DeviceBackend::PrecondModel &pm = *fn.pm;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    const unsigned long long nl = sh->n_local;
+    const int grid = grid_for(nl, pm.sms);
+    pm.shard = *sh;
+    cudaError_t e = cudaSuccess;
+    // dx once per point: the nested driver evaluates the objective and then the constraints at the same x
+    if (fn.row0 == 0 || pm.dx_of != x) {
+        e = launch_precond_dx(x, pm.x0, nl, pm.dx, grid, s);
+        ++pm.launches;
+    }
+    pm.dx_of = fn.row0 == 0 ? x : nullptr;
+    for (unsigned r = 0; r < m; ++r) {
+        const unsigned row = fn.row0 + r;
+        const FuncSpec &f = *pm.rows[row];
+        if (!f.dpre) continue;
+        double *h = pm.hdx + (size_t) pm.hrow[row] * ld;
+        const double t0 = wall_seconds();
+        f.dpre(sh, pm.x0, pm.dx, h, f.pre_data, stream);
+        pm.cb_seconds += wall_seconds() - t0;
+        if (row == 0 && pm.negate_h0) {
+            negate_kernel<<<grid_for((nl + 1) / 2, pm.sms), kBlock, 0, s>>>(h, nl);
+            ++pm.launches;
+        }
+    }
+    for (unsigned r = 0; r < m; ++r) {
+        const unsigned row = fn.row0 + r;
+        const int hr = pm.hrow[row];
+        const double *dfdx = row == 0 ? pm.g : pm.G + (size_t) (row - 1) * pm.ld0;
+        const double rho = row == 0 ? pm.rho : pm.rhoc[row - 1];
+        const cudaError_t em = launch_precond_model(pm.dx, pm.sigma, dfdx, hr < 0 ? nullptr : pm.hdx + (size_t) hr * ld, rho, nl,
+                                                    terms + (size_t) r * ld, hr < 0 ? nullptr : pm.qterms + (size_t) hr * ld,
+                                                    grad ? grad + (size_t) r * ld : nullptr, grid, s);
+        if (e == cudaSuccess) e = em;
+        ++pm.launches;
+        if (hr < 0 || sh->groups_local == 0) continue;
+        const cudaError_t ez = cudaMemsetAsync(pm.qsums + (size_t) row * kV, 0, kV * sizeof(double), s);
+        if (e == cudaSuccess) e = ez;
+        terms_group_kernel<<<dim3(sh->groups_local, 1), kTermsThreads, 0, s>>>(*sh, pm.qterms + (size_t) hr * ld, ld, pm.qpart);
+        nlopt_b200::detail::fold_groups_mkernel<<<dim3(sh->local_vshards, 1), kTermsThreads, 0, s>>>(
+            pm.qpart, sh->groups_local, sh->groups_per_vshard, pm.qsums + (size_t) row * kV + sh->vshard0);
+        pm.launches += 2;
+    }
+    // the quadratic sums of this callback's rows reach the host with the library's copy of the point's values
+    const cudaError_t ec = cudaMemcpyAsync(pm.qsums_host + (size_t) fn.row0 * kV, pm.qsums + (size_t) fn.row0 * kV,
+                                           (size_t) m * kV * sizeof(double), cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = ec;
+    if (e == cudaSuccess) e = cudaGetLastError();
+    if (pm.cuda == cudaSuccess) pm.cuda = e;
+}
+
+// value of row `row` from its separable total: (f + S) + Q
+double model_value(const DeviceBackend::PrecondModel &pm, unsigned row, double total)
+{
+    const double f = row == 0 ? pm.fval : pm.fcval[row - 1];
+    const double v = f + total;
+    return pm.hrow[row] < 0 ? v : v + shard_total(pm.qsums_host + (size_t) row * kV);
+}
+
+double model_finish(double total, void *data)
+{
+    return model_value(*static_cast<DeviceBackend::ModelFn *>(data)->pm, 0, total);
+}
+
+void model_mfinish(unsigned m, const double *totals, double *result, void *data)
+{
+    const DeviceBackend::PrecondModel &pm = *static_cast<DeviceBackend::ModelFn *>(data)->pm;
+    for (unsigned i = 0; i < m; ++i) result[i] = model_value(pm, 1 + i, totals[i]);
+}
+
+}  // namespace
+
+// A backend set up on device bounds and a device start point (model_solve's nested backend) takes new ones: the copies
+// and the start-point check of setup(), then the state of a fresh run (xcur == x, no mirrored point).
+bool DeviceBackend::rebind(const double *lb_dev, const double *ub_dev, double *x_dev, StartCheck *out)
+{
+    const size_t nl = geo_.n_local;
+    NB_CUDA(cudaMemcpyAsync(lb_, lb_dev, nl * sizeof(double), cudaMemcpyDeviceToDevice, stream_));
+    NB_CUDA(cudaMemcpyAsync(ub_, ub_dev, nl * sizeof(double), cudaMemcpyDeviceToDevice, stream_));
+    NB_CUDA(cudaMemcpyAsync(x_, x_dev, nl * sizeof(double), cudaMemcpyDeviceToDevice, stream_));
+    if (!rep_dev_ && (!small_dev((void **) &rep_dev_, sizeof(BoundsReport)) || !small_pinned((void **) &rep_host_, sizeof(BoundsReport))))
+        return false;
+    NB_CUDA(enqueue_bounds_check(lb_, ub_, x_, (unsigned) nl, rep_dev_, rep_host_, sm_count_, stream_));
+    ++stats_->kernel_launches;
+    NB_CUDA(cudaStreamSynchronize(stream_));
+    read_bounds_report(*rep_host_, out);
+    scalar_bounds_ = rep_host_->nonuniform == 0;
+    lb_u_ = scalar_bounds_ ? rep_host_->lb0 : 0.0;
+    ub_u_ = scalar_bounds_ ? rep_host_->ub0 : 0.0;
+    cfg_.lb_dev = lb_dev;
+    cfg_.ub_dev = ub_dev;
+    cfg_.x_dev = x_dev;
+    cand_in_x_ = true;
+    ++x_epoch_;
+    return true;
+}
+
+bool DeviceBackend::model_solve(const DualScalars &sc, const ModelStop &st, double *gval, double *gc, double *wval, int *ret,
+                                long long *nevals)
+{
+    const size_t nl = geo_.n_local, ld = geo_.ld;
+    PrecondModel &pm = model_;
+    if (!pre_lb_) {                                  // first model solve of the run
+        const size_t rows = 1 + (size_t) m_;
+        if (!small_dev((void **) &pre_lb_, ld * sizeof(double)) || !small_dev((void **) &pre_ub_, ld * sizeof(double)) ||
+            !small_dev((void **) &pm.dx, ld * sizeof(double)) ||
+            !small_dev((void **) &pm.hdx, (size_t) pm.npre * ld * sizeof(double)) ||
+            !small_dev((void **) &pm.qterms, (size_t) pm.npre * ld * sizeof(double)) ||
+            !small_dev((void **) &pm.qsums, rows * kV * sizeof(double)) ||
+            !small_pinned((void **) &pm.qsums_host, (rows + 1) * kV * sizeof(double)))
+            return false;
+        // the nested backend's groups (its geometry: n and the default chunking, one rank)
+        const Geometry ng = Geometry::make(geo_.n, 1, 0, kDefaultTargetChunks, kDefaultPmax);
+        pm.qpart_cap = ng.nseg_local > geo_.nseg_local ? ng.nseg_local : geo_.nseg_local;
+        if (!small_dev((void **) &pm.qpart, (pm.qpart_cap ? pm.qpart_cap : 1) * sizeof(double))) return false;
+    }
+    pm.x0 = x_;
+    pm.sigma = sigma_;
+    pm.g = g_;
+    pm.G = G_;
+    pm.ld0 = ld;
+    pm.fval = sc.fval;
+    pm.rho = sc.rho;
+    pm.fcval.assign(sc.fcval, sc.fcval + m_);
+    pm.rhoc.assign(sc.rhoc, sc.rhoc + m_);
+    pm.cuda = cudaSuccess;
+    pm.launches = 0;
+    pm.cb_seconds = 0;
+    pm.dx_of = nullptr;
+
+    // the trust box and the start point xcur = x (:441-446)
+    NB_CUDA(launch_precond_box(scalar_bounds_ ? nullptr : lb_, scalar_bounds_ ? nullptr : ub_, lb_u_, ub_u_, x_, sigma_, nl, pre_lb_,
+                               pre_ub_, xcur_, grid_for(nl, sm_count_), stream_));
+    ++stats_->kernel_launches;
+    cand_in_x_ = false;
+    ++x_epoch_;
+    NB_CUDA(cudaStreamSynchronize(stream_));        // the nested backend reads them on its own stream
+
+    // the nested LD_MMA run (:447-464): model objective and constraints, device bounds, device x, the dual tolerances.
+    // One nested backend (state, stream, workspace) serves every model solve of the run; each solve rebinds it to the new
+    // box and start point.
+    StartCheck start;
+    nested_stats_ = nlopt_b200_stats{};
+    if (!nested_) {
+        BackendConfig nc;
+        nc.variant = kMMA;
+        nc.n = geo_.n;
+        nc.objective.dtf = model_terms;
+        nc.objective.dfin = model_finish;
+        nc.objective.data = &model_fn_[0];
+        if (m_) {
+            FuncSpec c;
+            c.m = m_;
+            c.dtf = model_terms;
+            c.dmfin = model_mfinish;
+            c.data = &model_fn_[1];
+            nc.constraints.push_back(c);
+        }
+        nc.lb_dev = pre_lb_;
+        nc.ub_dev = pre_ub_;
+        nc.start_check = &start;
+        nc.x_dev = xcur_;
+        nc.stats = &nested_stats_;
+        nested_.reset(new DeviceBackend());
+        if (!nested_->setup(nc)) {
+            const std::string e = nested_->error();
+            nested_.reset();
+            return fail("nested model solve: " + e);
+        }
+    } else if (!nested_->rebind(pre_lb_, pre_ub_, xcur_, &start))
+        return fail("nested model solve: " + nested_->error());
+    DeviceBackend &nb = *nested_;
+    const nlopt_b200_stats &nst = nested_stats_;
+    auto settle = [&]() {
+        stats_->kernel_launches += nst.kernel_launches + pm.launches;
+        stats_->dual_operand_bytes += nst.dual_operand_bytes;
+        stats_->h2d_bytes += nst.h2d_bytes;
+        stats_->d2h_bytes += nst.d2h_bytes;
+        cb_seconds_ += pm.cb_seconds;
+        pm.launches = 0;
+        pm.cb_seconds = 0;
+    };
+    *nevals = 0;
+    if (start.bad >= 0) {                            // optimize.c:547-551 in the nested run (a NaN in the box)
+        char buf[160];
+        std::snprintf(buf, sizeof buf, "bounds %d fail %g <= %g <= %g", (int) start.bad, start.lb, start.x, start.ub);
+        err_ = buf;
+        *ret = kRetInvalid;
+        settle();
+        return true;
+    }
+    StopCriteria ns;
+    ns.ftol_rel = st.ftol_rel;
+    ns.ftol_abs = st.ftol_abs;
+    ns.maxeval = st.maxeval;
+    ns.maxtime = st.maxtime;
+    ns.force_stop = st.force_stop;
+    int nevals_nested = 0;
+    ns.nevals_p = &nevals_nested;
+    const std::vector<double> tol(m_, 0.0);
+    DriverStats ds;
+    std::string err;
+    double minf = HUGE_VAL;
+    const int r = ccsa_minimize(kMMA, nb, tol, &minf, ns, CcsaParams(), &ds, &err);
+    *nevals = ds.dual_evals;
+    *ret = r;
+    if (pm.cuda != cudaSuccess) { settle(); return fail("model function", pm.cuda); }
+    if (r < 0 || r == kRetMaxtime) {
+        err_ = err;
+        settle();
+        return true;
+    }
+    // xcur <- the nested optimum; g0, gi there (:465-467), from the nested backend, whose accepted point it is
+    bool ok = nb.fetch_x(xcur_) && nb.eval_objective(kBase, false, gval);
+    for (unsigned ic = 0; ok && ic < nb.num_constraint_objects(); ++ic) ok = nb.eval_constraint(kBase, ic, 0, false, gc);
+    ok = ok && nb.finish_evals(gval, gc);
+    settle();
+    if (!ok) return fail("nested model solve: " + nb.error());
+    if (pm.cuda != cudaSuccess) return fail("model function", pm.cuda);
+    // w = sum 1/2 ((xcur - x) / sigma)^2, reduced in the order of the model's sums
+    const nlopt_b200_shard &sh = pm.shard;
+    double *wsums = pm.qsums_host + (1 + (size_t) m_) * kV;
+    std::memset(wsums, 0, kV * sizeof(double));
+    if (sh.groups_local) {
+        NB_CUDA(launch_precond_w(xcur_, x_, sigma_, nl, pm.qterms, grid_for(nl, sm_count_), stream_));
+        NB_CUDA(cudaMemsetAsync(pm.qsums, 0, kV * sizeof(double), stream_));
+        terms_group_kernel<<<dim3(sh.groups_local, 1), kTermsThreads, 0, stream_>>>(sh, pm.qterms, ld, pm.qpart);
+        nlopt_b200::detail::fold_groups_mkernel<<<dim3(sh.local_vshards, 1), kTermsThreads, 0, stream_>>>(
+            pm.qpart, sh.groups_local, sh.groups_per_vshard, pm.qsums + sh.vshard0);
+        stats_->kernel_launches += 3;
+        NB_CUDA(cudaGetLastError());
+        NB_CUDA(cudaMemcpyAsync(wsums, pm.qsums, kV * sizeof(double), cudaMemcpyDeviceToHost, stream_));
+        NB_CUDA(cudaStreamSynchronize(stream_));
+    }
+    *wval = shard_total(wsums);
     return true;
 }
 

@@ -3,6 +3,7 @@
 
 #include <cuda_runtime.h>
 
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -28,6 +29,7 @@ public:
 
     bool setup(const BackendConfig &cfg);           // allocate + upload bounds/start point
     bool setup_raw(Variant v, unsigned n, unsigned m);   // kernel-level handle: arrays only
+    bool rebind(const double *lb_dev, const double *ub_dev, double *x_dev, StartCheck *out);   // new device bounds + x
 
     // ---- Backend ----
     unsigned n() const override { return (unsigned) geo_.n; }
@@ -51,6 +53,9 @@ public:
     bool supports_dual_solve() const override;
     bool dual_solve(double *y, const double *lo, const double *hi, const double *stop6, const DualScalars &sc, DualSums *out,
                     int *ret, long *nevals) override;
+    bool solves_model() const override { return model_.on; }
+    bool model_solve(const DualScalars &sc, const ModelStop &stop, double *gval, double *gc, double *wval, int *ret,
+                     long long *nevals) override;
     void accept_candidate() override;
     bool first_outer() override;
     bool end_outer(unsigned k, double sigma_min, double *dnorm, double *xnorm, bool *all_below_abs) override;
@@ -104,6 +109,37 @@ private:
     void release_small(void *p);
 
     BackendConfig cfg_;
+    // Preconditioned CCSAQ with device preconditioners (model_solve): what the model functions of the nested LD_MMA run
+    // (device_backend.cu: model_terms / model_finish) read of this backend, and their buffers.  Row 0 is the objective,
+    // row 1 + i constraint row i; hrow[r] indexes the Hdx / Q-term rows of a preconditioned row, -1 for the others.
+public:
+    struct PrecondModel {
+        bool on = false;
+        std::vector<const FuncSpec *> rows;
+        std::vector<int> hrow;
+        unsigned npre = 0;
+        bool negate_h0 = false;                      // a maximised objective: its preconditioner's H changes sign
+        const double *x0 = nullptr, *sigma = nullptr, *g = nullptr, *G = nullptr;
+        size_t ld0 = 0;                              // row stride of G
+        double fval = 0, rho = 0;
+        std::vector<double> fcval, rhoc;
+        const double *dx_of = nullptr;               // the x that dx belongs to (set by the objective's callback)
+        double *dx = nullptr, *hdx = nullptr, *qterms = nullptr, *qpart = nullptr, *qsums = nullptr, *qsums_host = nullptr;
+        size_t qpart_cap = 0;
+        nlopt_b200_shard shard{};                    // the nested run's geometry (the order of its sums)
+        int sms = 132;
+        long long launches = 0;
+        double cb_seconds = 0;                       // inside the preconditioners
+        cudaError_t cuda = cudaSuccess;              // the first launch error inside a model function
+    };
+    struct ModelFn { PrecondModel *pm; unsigned row0; };
+private:
+    PrecondModel model_;
+    ModelFn model_fn_[2];
+    double *pre_lb_ = nullptr, *pre_ub_ = nullptr;
+    std::unique_ptr<DeviceBackend> nested_;          // the nested LD_MMA run's backend, kept for the whole run
+    nlopt_b200_stats nested_stats_{};                // its statistics of the current model solve
+    struct BoundsReport *rep_dev_ = nullptr, *rep_host_ = nullptr;   // rebind(): the start-point check's report
     Variant variant_ = kMMA;
     unsigned m_ = 0;
     Geometry geo_;

@@ -463,6 +463,43 @@ nlopt_result nlopt_b200_set_min_objective_sharded(nlopt_opt opt, nlopt_b200_sfun
 nlopt_result nlopt_b200_set_max_objective_sharded(nlopt_opt opt, nlopt_b200_sfunc f, void *d)
 { return set_objective_checked(opt, sharded_spec(f, d), 1); }
 
+/* device preconditioners (nlopt_b200_dprecond): attached to a registered record of one row that has no host one */
+static nlopt_result set_dprecond(nlopt_opt opt, FuncSpec &fn, nlopt_b200_dprecond pre, void *pre_data)
+{
+    if (pre && fn.pre) {
+        set_err(opt, "this function has a host preconditioner (nlopt_precond); a function takes one preconditioner");
+        return NLOPT_INVALID_ARGS;
+    }
+    fn.dpre = pre;
+    fn.pre_data = pre ? pre_data : nullptr;
+    return NLOPT_SUCCESS;
+}
+
+nlopt_result nlopt_b200_set_objective_precond_device(nlopt_opt opt, nlopt_b200_dprecond pre, void *pre_data)
+{
+    if (!opt) return NLOPT_INVALID_ARGS;
+    clear_err(opt);
+    if (opt->objective.empty()) { set_err(opt, "no objective registered"); return NLOPT_INVALID_ARGS; }
+    return set_dprecond(opt, opt->objective, pre, pre_data);
+}
+
+nlopt_result nlopt_b200_set_constraint_precond_device(nlopt_opt opt, unsigned index, nlopt_b200_dprecond pre, void *pre_data)
+{
+    if (!opt) return NLOPT_INVALID_ARGS;
+    clear_err(opt);
+    if (index >= opt->fc.size()) {
+        set_err(opt, "inequality constraint index %u out of range (%u records; equality constraints take no preconditioner)",
+                index, (unsigned) opt->fc.size());
+        return NLOPT_INVALID_ARGS;
+    }
+    FuncSpec &fn = opt->fc[index].fn;
+    if (fn.m != 1) {
+        set_err(opt, "inequality constraint %u has %u rows: a vector constraint takes no preconditioner", index, fn.m);
+        return NLOPT_INVALID_ARGS;
+    }
+    return set_dprecond(opt, fn, pre, pre_data);
+}
+
 nlopt_algorithm nlopt_get_algorithm(const nlopt_opt opt) { return opt->algorithm; }
 unsigned nlopt_get_dimension(const nlopt_opt opt) { return opt->n; }
 const char *nlopt_get_errmsg(nlopt_opt opt) { return opt->has_errmsg ? opt->errmsg.c_str() : nullptr; }
@@ -1093,10 +1130,17 @@ nlopt_result run_ccsa(nlopt_opt opt, double *x_host, double *x_dev, double *minf
     prm.dual_xtol_abs = nlopt_get_param(opt, "dual_xtol_abs", 0.0);
     prm.dual_maxeval = (int) nlopt_get_param(opt, "dual_maxeval", lo ? (double) lo->maxeval : 100000.0);
 
-    bool any_pre = opt->objective.pre != nullptr, all_host = opt->objective.host();
+    bool any_pre = opt->objective.pre != nullptr, all_host = opt->objective.host(), any_dpre = opt->objective.dpre != nullptr;
     for (const auto &c : opt->fc) {
         any_pre = any_pre || c.fn.pre != nullptr;
+        any_dpre = any_dpre || c.fn.dpre != nullptr;
         all_host = all_host && c.fn.host();
+    }
+    any_dpre = any_dpre && opt->algorithm == NLOPT_LD_CCSAQ;     /* LD_MMA ignores preconditioners (mma.c) */
+    if (any_pre && any_dpre) {
+        set_err(opt, "preconditioned CCSAQ takes host preconditioners (nlopt_precond) or device preconditioners "
+                     "(nlopt_b200_dprecond), not both in one run");
+        return NLOPT_INVALID_ARGS;
     }
     if (any_pre && opt->algorithm == NLOPT_LD_CCSAQ) {          /* ccsa_quadratic.c: the !no_precond branch */
         if (!x_host || !all_host) {
@@ -1117,6 +1161,9 @@ nlopt_result run_ccsa(nlopt_opt opt, double *x_host, double *x_dev, double *minf
     cfg.n = n;
     cfg.objective = opt->objective;
     cfg.penalty = opt->penalty;
+    /* a maximisation reaches here as the minimisation of -f: a host objective wrapped in flipped(), any other form
+       with FuncSpec::negate (optimize_common) */
+    cfg.maximize = opt->objective.negate || opt->objective.f == flipped;
     std::vector<double> tol;
     for (const auto &c : opt->fc) {
         cfg.constraints.push_back(c.fn);
@@ -1166,6 +1213,16 @@ nlopt_result run_ccsa(nlopt_opt opt, double *x_host, double *x_dev, double *minf
         delete be;
         set_err(opt, "bounds %d fail %g <= %g <= %g", (int) start.bad, start.lb, start.x, start.ub);
         return NLOPT_INVALID_ARGS;
+    }
+    if (any_dpre && be->ranks() > 1) {               /* the nested model solve runs on device bounds: one rank */
+        delete be;
+        set_err(opt, "preconditioned CCSAQ with device preconditioners runs on one GPU in this library");
+        return NLOPT_INVALID_ARGS;
+    }
+    if (any_dpre && !be->solves_model()) {           /* never a silent separable run */
+        delete be;
+        set_err(opt, "this backend does not solve preconditioned models");
+        return NLOPT_FAILURE;
     }
     opt->stats.seconds_setup = nb200::wall_seconds() - t0;
 
@@ -1606,6 +1663,7 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
        objective, the rest as the penalty spec */
     sub->objective = opt->objective;    /* negate too: a maximised device objective's sub-problem L starts from -f */
     sub->objective.pre = nullptr;       /* auglag.c:109-135: the sub-problem takes no preconditioner */
+    sub->objective.dpre = nullptr;
     sub->maximize = 0;
     if (dev_bounds) {                                /* D2D into the sub-optimiser, which is then in device mode */
         std::string err;
@@ -1634,6 +1692,7 @@ nlopt_result run_auglag(nlopt_opt opt, double *x, double *x_dev, double *minf)
     for (const auto &c : sub_fc) {
         FuncSpec fn = c.fn;
         fn.pre = nullptr;                   /* as the objective's */
+        fn.dpre = nullptr;
         const nlopt_result r = add_any(sub, false, fn, c.tol.data());
         if (r < 0) return r;
     }

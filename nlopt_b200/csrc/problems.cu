@@ -137,6 +137,26 @@ struct AddBlockMean {
 
 }  // namespace
 
+// Tridiagonal preconditioner vpre = sign * A v, A = tridiag(-1, d_j, -1) (tests/test_host_driver.py: precond_problem;
+// sign -1 for the maximisation of the negated problem), one rank.  The operations are those of the PyTorch form
+// ((d_j v_j - v_{j+1}) - v_{j-1}, then the sign), so both give the same bits.
+struct nb200p_tridiag_data {
+    const double *d;     // device, n entries
+    double sign;
+};
+
+__global__ void nb200p_tridiag_kernel(const double *__restrict__ d, const double *__restrict__ v, double sign,
+                                      unsigned long long n, double *__restrict__ vpre)
+{
+    for (unsigned long long j = (unsigned long long) blockIdx.x * blockDim.x + threadIdx.x; j < n;
+         j += (unsigned long long) gridDim.x * blockDim.x) {
+        double o = __dmul_rn(d[j], v[j]);
+        if (j + 1 < n) o = __dsub_rn(o, v[j + 1]);
+        if (j > 0) o = __dsub_rn(o, v[j - 1]);
+        vpre[j] = __dmul_rn(sign, o);
+    }
+}
+
 extern "C" {
 
 nb200p_problem_s *nb200p_create(void) { return new nb200p_problem_s; }
@@ -448,6 +468,17 @@ void *nb200p_make_linear_data(nb200p_problem_s *p, const double *w_host, double 
     nb200p_lin_data *d = new nb200p_lin_data{w_host, b};
     p->lin_host.push_back(d);
     return d;
+}
+
+// an nlopt_b200_dprecond; data: an nb200p_tridiag_data in host memory
+void nb200p_tridiag_precond(const nlopt_b200_shard *shard, const double *x, const double *v, double *vpre, void *data,
+                            void *stream)
+{
+    (void) x;
+    const nb200p_tridiag_data &t = *static_cast<const nb200p_tridiag_data *>(data);
+    const unsigned long long n = shard->n_local;
+    const unsigned long long g = (n + 255) / 256;
+    nb200p_tridiag_kernel<<<(int) (g < 1 ? 1 : g > 4096 ? 4096 : g), 256, 0, static_cast<cudaStream_t>(stream)>>>(t.d, v, t.sign, n, vpre);
 }
 
 }  // extern "C"
